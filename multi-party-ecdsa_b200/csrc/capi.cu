@@ -470,7 +470,9 @@ int launch_nadic_shape(tecdsa_ctx* c, const ExpLaunch& l) {
     char* d_desc; unsigned int* d_counter; uint32_t* d_tables;
     int rc = job_prepare(c, table_bytes, &l, sizeof(ExpLaunch), &d_desc, &d_counter, &d_tables);
     if (rc) return rc;
-    c->prof_begin(K == 64 ? (TPI == 8 ? "nadic_jobs_kernel<64,8>" : "nadic_jobs_kernel<64,4>") : (TPI == 4 ? "nadic_jobs_kernel<32,4>" : "nadic_jobs_kernel<32,2>"));
+    // the profile keeps the pointer: one static label per instantiation, naming all three parameters so every shape is told apart
+    static const struct Label { char s[48]; Label() { snprintf(s, sizeof(s), "nadic_jobs_kernel<%d,%d,%d>", K, TPI, MINB); } } label;
+    c->prof_begin(label.s);
     nadic_jobs_kernel<K, TPI, MINB><<<grid, JOB_BLOCK, 0, c->stream>>>(reinterpret_cast<const ExpLaunch*>(d_desc), d_tables, d_counter, c->d_work);
     c->prof_end();
     c->count_launch();
