@@ -55,6 +55,10 @@ struct tecdsa_keyset {
     uint32_t* nadic = nullptr;   // [rows][10*64] N-adic constants of the Paillier moduli N, see nadic.cuh
     uint32_t* nadic_p = nullptr; // [rows][10*32] the same for the primes p and q (jobs modulo p^2, q^2)
     uint32_t* nadic_q = nullptr;
+    // sliding-window digits (recode.h) of the exponents N, p, q, p-1, q-1: rec[t] = [rows][32 * KEY_SIZE[t]] bytes inside
+    // rec_mem, nullptr for the other tables
+    uint8_t* rec_mem = nullptr;
+    const uint8_t* rec[tecdsa::KT_COUNT] = {};
     int n_keysets = 0;
 };
 

@@ -8,6 +8,7 @@
 #include "ctx.h"
 #include "gg20_rounds.cuh"
 #include "modinv.cuh"
+#include "recode.h"
 
 #include <cstdlib>
 #include <string>
@@ -25,6 +26,7 @@ struct Builder {
     int U;
     ExpLaunch L32, L64, L128, LPQ;      // 1024-bit, 2048-bit, N-adic mod N^2, p-adic mod p^2 / q^2
     InvLaunch I64, I128, I128H;        // I128H: modulo N^2 via the N-wide inversion + Hensel step
+    const uint32_t *ord_own, *ord_peer; // the units sorted by own / peer key row
 
     Operand fld(int f, int limbs = 0) const {
         return Operand{A.base + (size_t)A.off[f] * U, nullptr, A.size[f], 0, (uint32_t)(limbs ? limbs : A.size[f])};
@@ -61,6 +63,16 @@ struct Builder {
         k.mul[0] = m0; k.mul[1] = m1; k.mul[2] = m2; k.nbases = nb; k.nmul = nm; k.wide0 = wide0;
         k.fb = nullptr; k.fb_row = Operand{nullptr, nullptr, 0, 0, 0}; k.fb_sel[0] = k.fb_sel[1] = 0;
         k.nadic = nadic;
+        // base 0 raised to a recoded key constant (N, p, q, p-1, q-1 of the own or the peer's row): sliding windows, with the
+        // instances in key-row order so that whole warps share the digits
+        k.rec = Operand{nullptr, nullptr, 0, 0, 0}; k.order = nullptr;
+        const uint32_t* ord = e0.idx == A.row_own ? ord_own : e0.idx == A.row_peer ? ord_peer : nullptr;
+        for (int t = 0; t < KT_COUNT; t++)
+            if (nadic.ptr && nb > 0 && ord && ks->rec[t] && e0.ptr == A.key[t] && el0 == KEY_SIZE[t]) {
+                const uint32_t words = 8 * KEY_SIZE[t];
+                k.rec = Operand{reinterpret_cast<const uint32_t*>(ks->rec[t]), e0.idx, words, 1, words};
+                k.order = ord;
+            }
         k.out = out(out_field); k.out_stride = A.size[out_field]; k.count = U; k.item_begin = dst->total_items;
         dst->total_items += (U + gpw - 1) / gpw;
     }
@@ -205,6 +217,25 @@ extern "C" int tecdsa_keys_upload(tecdsa_ctx* c, const tecdsa_keys* k, tecdsa_ke
         if (!rc) rc = c->nadic_setup(ks->tab[KT_Q], ks->nadic_q, rows, 32);
         if (rc) { tecdsa_keys_free(c, ks); return rc; }
     }
+    {   // sliding-window digits of the exponents that are per-key constants (recode.h); N comes back from gg20_key_setup
+        std::vector<uint32_t> n_host((size_t)rows * 64), pm1(k->paillier_p, k->paillier_p + (size_t)rows * 32), qm1(k->paillier_q, k->paillier_q + (size_t)rows * 32);
+        CK(cudaMemcpyAsync(n_host.data(), ks->tab[KT_N], n_host.size() * 4, cudaMemcpyDeviceToHost, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        for (int r = 0; r < rows; r++) { pm1[(size_t)r * 32] ^= 1u; qm1[(size_t)r * 32] ^= 1u; }      // odd primes: p-1 clears bit 0
+        const struct { int t; const uint32_t* e; } ex[] = {{KT_N, n_host.data()}, {KT_P, k->paillier_p}, {KT_Q, k->paillier_q},
+                                                            {KT_PM1, pm1.data()}, {KT_QM1, qm1.data()}};
+        size_t offs[5], bytes = 0;
+        for (int x = 0; x < 5; x++) { offs[x] = bytes; bytes += (size_t)rows * 32 * KEY_SIZE[ex[x].t]; }
+        std::vector<uint8_t> digits(bytes);
+        for (int x = 0; x < 5; x++) {
+            const int limbs = KEY_SIZE[ex[x].t];
+            for (int r = 0; r < rows; r++) slide_recode(digits.data() + offs[x] + (size_t)r * 32 * limbs, ex[x].e + (size_t)r * limbs, limbs);
+        }
+        CK(cudaMalloc(&ks->rec_mem, bytes));
+        CK(cudaMemcpyAsync(ks->rec_mem, digits.data(), bytes, cudaMemcpyHostToDevice, c->stream));
+        CK(cudaStreamSynchronize(c->stream));
+        for (int x = 0; x < 5; x++) ks->rec[ex[x].t] = ks->rec_mem + offs[x];
+    }
     CK(cudaStreamSynchronize(c->stream));
 #undef CK
 #define CK(call)                                                               \
@@ -223,6 +254,7 @@ extern "C" int tecdsa_keys_free(tecdsa_ctx* c, tecdsa_keyset* ks) {
     if (ks->nadic) cudaFree(ks->nadic);
     if (ks->nadic_p) cudaFree(ks->nadic_p);
     if (ks->nadic_q) cudaFree(ks->nadic_q);
+    if (ks->rec_mem) cudaFree(ks->rec_mem);
     delete ks;
     return 0;
 }
@@ -256,8 +288,9 @@ static int offline_impl(tecdsa_ctx* c, const tecdsa_keyset* ks, const uint32_t* 
     const int U = (int)n_sessions * 2;
 
     // ---- host-side unit tables (who am I, who is my peer, which key rows)
-    std::vector<uint32_t> idx((size_t)7 * U);
+    std::vector<uint32_t> idx((size_t)9 * U);
     uint32_t *row_own = idx.data(), *row_peer = row_own + U, *row_st = row_peer + U, *peer = row_st + 3 * (size_t)U, *kset = peer + U;
+    uint32_t *ord_own = kset + U, *ord_peer = ord_own + U;
     for (size_t s = 0; s < n_sessions; s++) {
         uint32_t k = h_sess[3 * s], a = h_sess[3 * s + 1], b = h_sess[3 * s + 2];
         if (k >= (uint32_t)ks->n_keysets || a > 2 || b > 2 || a == b) return tecdsa_fail(TECDSA_E_ARG, "gg20_offline: bad session descriptor");
@@ -267,6 +300,15 @@ static int offline_impl(tecdsa_ctx* c, const tecdsa_keyset* ks, const uint32_t* 
             for (int x = 0; x < 3; x++) row_st[(size_t)x * U + u] = k * 3 + x;
             peer[u] = (uint32_t)(u ^ 1); kset[u] = k;
         }
+    }
+    // counting sorts of the units by own and by peer key row (stable): the instance order of the classes with recoded exponents
+    for (int side = 0; side < 2; side++) {
+        const uint32_t* row = side ? row_peer : row_own;
+        uint32_t* ord = side ? ord_peer : ord_own;
+        std::vector<uint32_t> next((size_t)ks->n_keysets * 3 + 1, 0);
+        for (int u = 0; u < U; u++) next[row[u] + 1]++;
+        for (size_t r = 1; r < next.size(); r++) next[r] += next[r - 1];
+        for (int u = 0; u < U; u++) ord[next[row[u]]++] = (uint32_t)u;
     }
     // ---- arena
     Builder B;
@@ -282,7 +324,8 @@ static int offline_impl(tecdsa_ctx* c, const tecdsa_keyset* ks, const uint32_t* 
     A.U = U;
     uint32_t* d_idx = reinterpret_cast<uint32_t*>(c->arena + ((arena_bytes + 255) & ~size_t(255)));
     A.row_own = d_idx; A.row_peer = d_idx + U; A.row_st = d_idx + 2 * (size_t)U; A.peer = d_idx + 5 * (size_t)U; A.keyset = d_idx + 6 * (size_t)U;
-    A.status = reinterpret_cast<uint8_t*>(d_idx + 7 * (size_t)U);
+    B.ord_own = d_idx + 7 * (size_t)U; B.ord_peer = d_idx + 8 * (size_t)U;
+    A.status = reinterpret_cast<uint8_t*>(d_idx + 9 * (size_t)U);
     for (int t = 0; t < KT_COUNT; t++) A.key[t] = ks->tab[t];
     A.ypk = ks->ypk;
     CK(cudaMemcpyAsync(d_idx, idx.data(), idx_bytes, cudaMemcpyHostToDevice, c->stream));
@@ -337,18 +380,18 @@ static int offline_impl(tecdsa_ctx* c, const tecdsa_keyset* ks, const uint32_t* 
     // peer's PDL proof in round 5 (declared shortcut, identical value)
     B.inv_class(I128, GPWI128, B.key(KT_NN, rp), B.peer(F_CK), F_CINVP, 3);
     RUN(run_inv(c, I128, 128)); RUN(run_inv(c, B.I128H, -128));
-    for (int x = 0; x < 3; x++) {
+    for (int x = 0; x < 3; x++)
         B.exp_class(L64, GPW64, B.key(KT_NT, st_rows(x)), 1, B.peer(F_Z0 + x), B.peer(F_E0 + x), 8, NONE, NONE, 0, 0, NONE, NONE, F_ZE0 + x);   // z^e (:122)
-        B.exp_class(L128, GPW128, B.key(KT_NN, rp), 1, B.fld(F_CINVP), B.peer(F_E0 + x), 8, NONE, NONE, 0, 0, NONE, NONE, F_CEI0 + x);           // (c^-1)^e (:135)
-    }
-    RUN(run_exp(c, L128, 128)); RUN(run_exp(c, B.LPQ, -32)); RUN(run_exp(c, L64, 64));
+    RUN(run_exp(c, L64, 64));
     for (int x = 0; x < 3; x++) B.inv_class(I64, GPW64, B.key(KT_NT, st_rows(x)), B.fld(F_ZE0 + x), F_ZEI0 + x, x);
     RUN(run_inv(c, I64, 64));
     for (int x = 0; x < 3; x++) {
         // w' = h1^s1 * h2^s2 * (z^e)^-1 mod N_tilde                     (range_proofs.rs:129-132)
         B.fb_class(L64, GPW64, st_rows(x), B.peer(F_S20 + x), 92, B.peer(F_S10 + x), 28, 1, B.fld(F_ZEI0 + x), F_WV0 + x);
-        // u' = (s1 N + 1) * s^N * (c^e)^-1 mod N^2                      (range_proofs.rs:134-141)
-        B.exp_class(L128, GPW128, B.key(KT_NN, rp), 1, B.peer(F_S0 + x, 64), B.key(KT_N, rp), 64, NONE, NONE, 0, 2, B.fld(F_GS10 + x), B.fld(F_CEI0 + x), F_UV0 + x);
+        // u' = (s1 N + 1) * s^N * (c^e)^-1 mod N^2                      (range_proofs.rs:134-141); (c^-1)^e (:135) is the second
+        // base of the same job and shares its squarings
+        B.exp_class(L128, GPW128, B.key(KT_NN, rp), 2, B.peer(F_S0 + x, 64), B.key(KT_N, rp), 64, B.fld(F_CINVP), B.peer(F_E0 + x), 8, 1,
+                    B.fld(F_GS10 + x), NONE, F_UV0 + x);
     }
     // c_b = c_a^b * Enc(beta'; r') mod N^2 for b = gamma_i and b = w_i  (mta/mod.rs:133-145)
     B.exp_class(L128, GPW128, B.key(KT_NN, rp), 2, B.rnd(RND_R_G, 64), B.key(KT_N, rp), 64, B.peer(F_CK), B.rnd(RND_GAMMA, 8), 8, 1, B.fld(F_LBG), NONE, F_CBG);
@@ -390,12 +433,12 @@ static int offline_impl(tecdsa_ctx* c, const tecdsa_keyset* ks, const uint32_t* 
     B.inv_class(I128, GPWI128, B.key(KT_NN, ro), B.fld(F_CK), F_CINVO, 8);          // own ciphertext (proof j = 0); the peer's inverse is CINVP
     RUN(run_inv(c, I128, 128)); RUN(run_inv(c, B.I128H, -128));
     for (int j = 0; j < 2; j++) {
-        const uint32_t* prover = j ? rp : ro;            // key row of the prover
         const uint32_t* stmt = j ? ro : rp;              // whose (N_tilde, h1, h2) the proof was made against
         Operand z = j ? B.peer(F_PZ) : B.fld(F_PZ);
         B.exp_class(L64, GPW64, B.key(KT_NT, stmt), 1, z, B.fld(F_VE0 + j), 8, NONE, NONE, 0, 0, NONE, NONE, F_VZE0 + j);       // z^e; (z^-1)^e == (z^e)^-1 (:166-172)
-        B.exp_class(L128, GPW128, B.key(KT_NN, prover), 1, B.fld(j ? F_CINVP : F_CINVO), B.fld(F_VE0 + j), 8, NONE, NONE, 0, 0, NONE, NONE, F_VCEI0 + j);  // (c^-1)^e (:151-157)
     }
+    // (c^-1)^e (:151-157) of the own proof; the peer's proof takes it as the second base of its u2' job below
+    B.exp_class(L128, GPW128, B.key(KT_NN, ro), 1, B.fld(F_CINVO), B.fld(F_VE0), 8, NONE, NONE, 0, 0, NONE, NONE, F_VCEI0);
     B.crt_stage1(L32, GPW32, ro, 5, B.fld(F_PS2, 64));       // own proof's s2^N mod N^2_own through the CRT stages
     RUN(run_exp(c, L32, 32));
     B.crt_stage2(L64, GPW64, ro, 5);
@@ -404,14 +447,14 @@ static int offline_impl(tecdsa_ctx* c, const tecdsa_keyset* ks, const uint32_t* 
     for (int j = 0; j < 2; j++) B.inv_class(I64, GPW64, B.key(KT_NT, j ? ro : rp), B.fld(F_VZE0 + j), F_VZEI0 + j, 6 + j);
     RUN(run_inv(c, I64, 64));
     for (int j = 0; j < 2; j++) {
-        const uint32_t* prover = j ? rp : ro;
+        const uint32_t* prover = j ? rp : ro;            // key row of the prover
         const uint32_t* stmt = j ? ro : rp;
         Operand s1 = j ? B.peer(F_PS1) : B.fld(F_PS1), s2 = j ? B.peer(F_PS2, 64) : B.fld(F_PS2, 64), s3 = j ? B.peer(F_PS3) : B.fld(F_PS3);
         // u3' = h1^s1 * h2^s3 * z^-e mod N_tilde                         (:158-172)
         B.fb_class(L64, GPW64, stmt, s3, 92, s1, 28, 1, B.fld(F_VZEI0 + j), F_VU30 + j);
         // u2' = (N+1)^s1 * s2^N * c^-e mod N^2                           (:144-157)
         if (j == 0) B.exp_class(L128, GPW128, B.key(KT_NN, prover), 0, NONE, NONE, 0, NONE, NONE, 0, 3, B.fld(F_VLIN0), B.fld(F_VCEI0), F_VU20, 0, B.fld(F_XC5));
-        else B.exp_class(L128, GPW128, B.key(KT_NN, prover), 1, s2, B.key(KT_N, prover), 64, NONE, NONE, 0, 2, B.fld(F_VLIN0 + j), B.fld(F_VCEI0 + j), F_VU20 + j);
+        else B.exp_class(L128, GPW128, B.key(KT_NN, prover), 2, s2, B.key(KT_N, prover), 64, B.fld(F_CINVP), B.fld(F_VE1), 8, 1, B.fld(F_VLIN1), NONE, F_VU21);
     }
     RUN(run_exp(c, L128, 128)); RUN(run_exp(c, B.LPQ, -32)); RUN(run_exp(c, L64, 64));
     RUN(glue(c, gg20_r5_check, A, 2));

@@ -62,6 +62,11 @@ struct ExpClass {
     // N-adic mode (nadic.cuh, nadic_jobs_kernel only): the job is modulo N^2, `mod` names N and this the key's
     // constants row (digits of R, R^2, R^3 mod N^2)
     Operand nadic;
+    // nadic_jobs_kernel only.  `rec`: sliding-window digits of exp[0] (recode.h, one byte per bit), for exponents that are
+    // a key row's constant; ptr nullptr = fixed windows.  `order`: instance g works on unit order[g] (nullptr = g); sorting
+    // the instances by that key row lets the lane groups of a warp share the digits.
+    Operand rec;
+    const uint32_t* order;
     int count;              // instances
     int item_begin;         // first warp-item of this class in the launch (prefix sum)
 };

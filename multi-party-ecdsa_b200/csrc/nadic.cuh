@@ -206,9 +206,9 @@ static constexpr int NADIC_CONST_K = 10;
 static constexpr int NADIC_TABLE_ENTRIES = 2 * (1 << WINDOW_BITS) + 1;  // per lane group: two window tables + one parked value, 2K limbs each
 
 // plain operand c = sum_h c_h R^h (up to 4K limbs, zero-extended from o.limbs, any value) -> Montgomery digits of c mod N^2:
-// sum_h (c_h, 0) * R^(h+2) * R^-1
+// sum_h (c_h, 0) * R^(h+2) * R^-1.  Returns the number of products (each without the second cross product).
 template <int TPI, int L>
-__device__ __forceinline__ void to_nadic(Dig<L>& X, const Operand& o, int i, const uint32_t* consts, const uint32_t (&n)[L], uint32_t n0inv) {
+__device__ __forceinline__ int to_nadic(Dig<L>& X, const Operand& o, int i, const uint32_t* consts, const uint32_t (&n)[L], uint32_t n0inv) {
     constexpr int K = TPI * L;
     Dig<L> a, c, part;
 #pragma unroll
@@ -222,6 +222,7 @@ __device__ __forceinline__ void to_nadic(Dig<L>& X, const Operand& o, int i, con
         nadic_mul<TPI, L>(part, a, c, false, n, n0inv);        // a.d1 == 0: no X1*Y0 term
         dig_add<TPI, L>(X, X, part, n);
     }
+    return parts;
 }
 
 // Same job semantics as exp_jobs_kernel (out = m1*m2*m3 * b1^e1 * b2^e2 mod N^2, plain 2K-limb operands and result), but
@@ -251,12 +252,22 @@ nadic_jobs_kernel(const ExpLaunch* __restrict__ launch, uint32_t* __restrict__ t
         const ExpClass& c = launch->cls[ci];
         const int g = ((int)item - c.item_begin) * GPW + lane / TPI;
         const bool live = g < c.count;
-        const int i = live ? g : c.count - 1;
+        const int gi = live ? g : c.count - 1;
+        const int i = c.order ? (int)__ldg(c.order + gi) : gi;     // the unit this lane group works on
 
         uint32_t n[L];
         load_operand<TPI, L>(n, c.mod, i);
         const uint32_t n0inv = neg_inv32(__shfl_sync(FULL, n[0], 0, TPI));
         const uint32_t* consts = operand_at(c.nadic, i);
+        // base 0 runs on its sliding-window digits only when every group of the warp has the same ones: the positions of
+        // the products depend on the digits, and every nadic_mul must be reached by all 32 lanes (it shuffles across the
+        // warp).  A warp that straddles two key rows takes fixed windows.
+        const uint8_t* dig = nullptr;
+        if (c.rec.ptr) {
+            const unsigned long long d = (unsigned long long)operand_at(c.rec, i);
+            if (__all_sync(FULL, d == __shfl_sync(FULL, d, 0))) dig = reinterpret_cast<const uint8_t*>(d);
+        }
+        uint32_t prods = 0;                                         // products run: low half without, high half with the second cross product
 
         // operands 0..nbases-1 are bases (window tables), the rest plain multipliers (folded into P)
         Dig<L> acc, Y;
@@ -268,58 +279,89 @@ nadic_jobs_kernel(const ExpLaunch* __restrict__ launch, uint32_t* __restrict__ t
 #pragma unroll 1
         for (int k = 0; k < c.nbases + c.nmul; k++) {
             const bool is_base = k < c.nbases;
+            const bool odd = k == 0 && dig;
             Dig<L> xr;
-            to_nadic<TPI, L>(xr, is_base ? c.base[k] : c.mul[k - c.nbases], i, consts, n, n0inv);
+            prods += to_nadic<TPI, L>(xr, is_base ? c.base[k] : c.mul[k - c.nbases], i, consts, n, n0inv);
             uint32_t* tb = my_tbl + (size_t)k * TBL * 2 * K;
-            if (is_base) {
+            // fixed windows: entry j = x^j, Y runs through x^2 .. x^31.  Sliding windows: entry j = x^(2j+1); the first step
+            // squares x, which then becomes the step, and Y runs through x^3 .. x^63.  Multiplier: one product P *= x.
+            int steps = 1, first = 0;
+            if (odd) {
+                store_dig<TPI, L>(tb, xr);
+                square_operand<TPI, L>(Y, xr, n);
+                steps = TBL;
+            } else if (is_base) {
                 load_dig<TPI, L>(Y, consts + NADIC_ONE * K);
                 store_dig<TPI, L>(tb, Y);
                 store_dig<TPI, L>(tb + 2 * K, xr);
                 Y = xr;
+                steps = TBL - 2; first = 2;
             } else {
                 load_dig<TPI, L>(Y, p_slot);
             }
-            // base: Y runs through xr^2 .. xr^31 into the table; multiplier: one product P *= xr
-            const int steps = is_base ? TBL - 2 : 1;
 #pragma unroll 1
             for (int e = 0; e < steps; e++) {
-                nadic_mul<TPI, L>(Y, Y, xr, true, n, n0inv);
-                if (is_base) store_dig<TPI, L>(tb + (size_t)(e + 2) * 2 * K, Y);
+                const bool sq = odd && e == 0;
+                nadic_mul<TPI, L>(Y, xr, Y, !sq, n, n0inv);
+                prods += sq ? 1u : 0x10000u;
+                if (sq) { xr = Y; load_dig<TPI, L>(Y, tb); }
+                else if (is_base) store_dig<TPI, L>(tb + (size_t)(e + first) * 2 * K, Y);
             }
             if (!is_base) store_dig<TPI, L>(p_slot, Y);
         }
         __syncwarp();
-        // exponentiation; the multiplier product P and the exit from the Montgomery domain (times (1, 0)) are the two
-        // last steps of the same loop
+        // exponentiation, one state per product from the top bit down: the squaring (once acc is no longer one), the digit
+        // of base 0, the window of base 1; then the multiplier product P and the exit from the Montgomery domain (times (1, 0)).
+        // A fixed window multiplies at its lowest bit, also when it is zero, so that the products stay warp-uniform.
         load_dig<TPI, L>(acc, consts + NADIC_ONE * K);
         {
-            const uint32_t* e0 = operand_at(c.exp[0], i);
-            const uint32_t* e1 = c.nbases > 1 ? operand_at(c.exp[1], i) : e0;
-            const int nw0 = c.nbases > 0 ? (c.exp_limbs[0] * 32 + WINDOW_BITS - 1) / WINDOW_BITS : 0;
+            // windows per base; the exponent addresses are re-read where a window is due, which keeps them out of the
+            // registers live across nadic_mul
+            const int nw0 = c.nbases > 0 && !dig ? (c.exp_limbs[0] * 32 + WINDOW_BITS - 1) / WINDOW_BITS : 0;
             const int nw1 = c.nbases > 1 ? (c.exp_limbs[1] * 32 + WINDOW_BITS - 1) / WINDOW_BITS : 0;
-            const int nw = nw0 > nw1 ? nw0 : nw1;
-            int w = nw - 1, ph = WINDOW_BITS;
+            int bit = (nw0 > nw1 ? nw0 : nw1) * WINDOW_BITS - WINDOW_BITS;
+            if (dig && c.exp_limbs[0] * 32 - 1 > bit) bit = c.exp_limbs[0] * 32 - 1;
+            if (bit < 0) bit = -1;
+            int ph = 1;
+            bool started = false;
 #pragma unroll 1
-            while (w >= -2) {
-                bool do_mul = true, cross2 = true;
-                if (w == -1) { load_dig<TPI, L>(Y, p_slot); do_mul = c.nmul > 0; w = -2; }
-                else if (w == -2) {
+            while (bit >= -2) {
+                bool do_mul = false, cross2 = true;
+                if (bit == -1) { load_dig<TPI, L>(Y, p_slot); do_mul = c.nmul > 0; bit = -2; }
+                else if (bit == -2) {
 #pragma unroll
                     for (int j = 0; j < L; j++) { Y.d0[j] = 0; Y.d1[j] = 0; }
                     if (gl == 0) Y.d0[0] = 1;
-                    w = -3;
+                    do_mul = true; bit = -3;
                 }
-                else if (ph < WINDOW_BITS) { square_operand<TPI, L>(Y, acc, n); cross2 = false; ph++; }
-                else if (ph == WINDOW_BITS) {
-                    if (w < nw0) load_dig<TPI, L>(Y, my_tbl + (size_t)exp_window(e0, c.exp_limbs[0], w) * 2 * K);
-                    else do_mul = false;
-                    ph++;
+                else if (ph == 0) {
+                    if (started) { square_operand<TPI, L>(Y, acc, n); cross2 = false; do_mul = true; }
+                    // straight on to the next bit's squaring where neither base can have a product at this one
+                    if (bit % WINDOW_BITS == 0 || (dig && __ldg(dig + bit))) ph = 1;
+                    else bit--;
+                } else if (ph == 1) {
+                    if (dig) {
+                        const uint32_t d = __ldg(dig + bit);
+                        if (d) { load_dig<TPI, L>(Y, my_tbl + (size_t)(d >> 1) * 2 * K); do_mul = true; }
+                    } else if (bit % WINDOW_BITS == 0 && bit / WINDOW_BITS < nw0) {
+                        const uint32_t win = exp_window(operand_at(c.exp[0], i), c.exp_limbs[0], bit / WINDOW_BITS);
+                        load_dig<TPI, L>(Y, my_tbl + (size_t)win * 2 * K);
+                        do_mul = true;
+                    }
+                    ph = 2;
                 } else {
-                    if (w < nw1) load_dig<TPI, L>(Y, my_tbl + ((size_t)TBL + exp_window(e1, c.exp_limbs[1], w)) * 2 * K);
-                    else do_mul = false;
-                    ph = 0; w--;
+                    if (bit % WINDOW_BITS == 0 && bit / WINDOW_BITS < nw1) {
+                        const uint32_t win = exp_window(operand_at(c.exp[1], i), c.exp_limbs[1], bit / WINDOW_BITS);
+                        load_dig<TPI, L>(Y, my_tbl + ((size_t)TBL + win) * 2 * K);
+                        do_mul = true;
+                    }
+                    ph = 0; bit--;
                 }
-                if (do_mul) nadic_mul<TPI, L>(acc, acc, Y, cross2, n, n0inv);
+                if (do_mul) {
+                    nadic_mul<TPI, L>(acc, acc, Y, cross2, n, n0inv);
+                    prods += cross2 ? 0x10000u : 1u;
+                    started = true;
+                }
             }
         }
         // plain value = d0 + d1 * N  (2K limbs)
@@ -334,27 +376,14 @@ nadic_jobs_kernel(const ExpLaunch* __restrict__ launch, uint32_t* __restrict__ t
             (void)group_add_masked<TPI, L>(hi, one, 0xffffffffu);
         }
         if (live) {
-            uint32_t* o = c.out + (size_t)g * c.out_stride;
+            uint32_t* o = c.out + (size_t)i * c.out_stride;
             store_limbs<TPI, L>(o, lo);
             store_limbs<TPI, L>(o + K, hi);
             if (gl == 0 && work) {
-                // nadic_mul: 4K^2 + 2K without the second cross product (lifts, squarings), 5K^2 + 2K with it
+                // nadic_mul: 4K^2 + 2K without the second cross product (lifts, squarings), 5K^2 + 2K with it; the exit ends
+                // with d0 + d1 * N (K^2)
                 const unsigned long long m4 = 4ull * K * K + 2 * K, m5 = 5ull * K * K + 2 * K;
-                unsigned long long macs = (unsigned long long)K * K + m5;                                    // exit: times (1, 0), then d0 + d1 * N
-                int nwmax = 0;
-                for (int k = 0; k < c.nbases + c.nmul; k++) {
-                    const Operand& o2 = k < c.nbases ? c.base[k] : c.mul[k - c.nbases];
-                    int parts = ((int)o2.limbs + K - 1) / K;
-                    macs += (unsigned long long)(parts > 4 ? 4 : parts) * m4;
-                    if (k < c.nbases) {
-                        const int nwb = (c.exp_limbs[k] * 32 + WINDOW_BITS - 1) / WINDOW_BITS;
-                        macs += (unsigned long long)(TBL - 2 + nwb) * m5;
-                        nwmax = nwb > nwmax ? nwb : nwmax;
-                    } else macs += m5;
-                }
-                if (c.nmul > 0) macs += m5;
-                if (nwmax > 0) macs += (unsigned long long)(nwmax - 1) * WINDOW_BITS * m4;
-                atomicAdd(work, macs);
+                atomicAdd(work, (unsigned long long)K * K + (prods & 0xffffu) * m4 + (prods >> 16) * m5);
             }
         }
         __syncwarp();
