@@ -372,10 +372,14 @@ int tecdsa_gg18_output_signature_batch(tecdsa_ctx* ctx, int parties, const uint3
  * A session is two units (2s, 2s+1); both run on the same GPU and exchange their messages in
  * device memory.  The LocalKey material (keygen/rounds.rs:310-322) is uploaded once per key
  * set; per-key constants (N^2, p^2, q^2, the CRT constants of Paillier decrypt) are derived
- * on the device.                                                                          */
+ * on the device.
+ * Accepted keys are those the reference's keygen accepts (gg_2020/party_i.rs:49-50, 287-290):
+ * odd p != q, both below 2^1024, with 2^2046 <= N = pq < 2^2048 (so each factor is above
+ * 2^1022 and p/q < 4), and 2^2046 <= N_tilde < 2^2048, odd.  Any other row makes
+ * tecdsa_keys_upload return TECDSA_E_ARG before anything is allocated.                    */
 typedef struct {
     size_t n_keysets;             /* rows below are indexed by keyset*3 + party (party 0..2)      */
-    const uint32_t* paillier_p;   /* [rows][32]  DecryptionKey.p  (1024-bit prime)                 */
+    const uint32_t* paillier_p;   /* [rows][32]  DecryptionKey.p  (odd prime, see above)           */
     const uint32_t* paillier_q;   /* [rows][32]  DecryptionKey.q                                   */
     const uint32_t* n_tilde;      /* [rows][64]  DLogStatement.N   (h1_h2_n_tilde_vec)             */
     const uint32_t* h1;           /* [rows][64]  DLogStatement.g                                   */

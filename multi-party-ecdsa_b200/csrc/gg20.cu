@@ -10,6 +10,7 @@
 #include "modinv.cuh"
 #include "recode.h"
 
+#include <algorithm>
 #include <cstdlib>
 #include <string>
 #include <thread>
@@ -18,6 +19,23 @@
 using namespace tecdsa;
 
 namespace {
+
+// bit length of a * b for two n-limb operands (n <= 32), by schoolbook product on the host
+int product_bits(const uint32_t* a, const uint32_t* b, int n) {
+    uint32_t prod[64] = {};
+    for (int i = 0; i < n; i++) {
+        uint64_t cy = 0;
+        for (int j = 0; j < n; j++) {
+            cy += (uint64_t)a[i] * b[j] + prod[i + j];
+            prod[i + j] = (uint32_t)cy;
+            cy >>= 32;
+        }
+        prod[i + n] = (uint32_t)cy;
+    }
+    for (int w = 2 * n - 1; w >= 0; w--)
+        if (prod[w]) return 32 * w + 32 - __builtin_clz(prod[w]);
+    return 0;
+}
 
 struct Builder {
     tecdsa_ctx* c;
@@ -165,10 +183,16 @@ extern "C" int tecdsa_keys_upload(tecdsa_ctx* c, const tecdsa_keys* k, tecdsa_ke
         return tecdsa_fail(TECDSA_E_ARG, "keys_upload: missing table");
     CK(cudaSetDevice(c->device));
     const int rows = (int)k->n_keysets * 3;
-    // every modulus must be odd (Montgomery domain): checked on the host copy BEFORE anything is allocated or launched
-    for (int r = 0; r < rows; r++)
-        if (!(k->paillier_p[(size_t)r * 32] & 1) || !(k->paillier_q[(size_t)r * 32] & 1) || !(k->n_tilde[(size_t)r * 64] & 1))
-            return tecdsa_fail(TECDSA_E_ARG, "keys_upload: even modulus");
+    // every modulus must be odd (Montgomery domain), and the key inside the domain of the header: checked on the host copy
+    // BEFORE anything is allocated or launched
+    for (int r = 0; r < rows; r++) {
+        const uint32_t *p = k->paillier_p + (size_t)r * 32, *q = k->paillier_q + (size_t)r * 32, *nt = k->n_tilde + (size_t)r * 64;
+        if (!(p[0] & 1) || !(q[0] & 1) || !(nt[0] & 1)) return tecdsa_fail(TECDSA_E_ARG, "keys_upload: even modulus");
+        if (std::equal(p, p + 32, q)) return tecdsa_fail(TECDSA_E_ARG, "keys_upload: p == q");
+        const int nb = product_bits(p, q, 32);
+        if (nb < 2047 || nb > 2048) return tecdsa_fail(TECDSA_E_ARG, "keys_upload: Paillier N outside [2^2046, 2^2048)");
+        if (!(nt[63] >> 30)) return tecdsa_fail(TECDSA_E_ARG, "keys_upload: N_tilde outside [2^2046, 2^2048)");
+    }
     tecdsa_keyset* ks = new tecdsa_keyset();
     ks->n_keysets = (int)k->n_keysets;
     // from here on every failure releases the partially built key set

@@ -150,12 +150,13 @@ static __device__ __noinline__ void decrypt_finish(uint32_t* m64, const Arena& A
         st::mul_low(lp, t, A.k(half ? KT_QINV2 : KT_PINV2, row), 32);
         st::mont_mul(half ? mq : mp, lp, A.k(half ? KT_HQR : KT_HPR, row), pr, st::neg_inv32_st(pr[0]), 32, scratch);
     }
-    // diff = (mq - mp) mod q
+    // diff = (mq - mp) mod q.  Accepted keys have 2^2046 <= pq and p, q < 2^1024 (tecdsa_keys_upload), so q > 2^1022 > p/4:
+    // mq - mp > -p > -4q, and at most 4 additions of q make it non-negative
     uint32_t diff[33], mpx[33], qx[33];
     for (int i = 0; i < 32; i++) { diff[i] = mq[i]; mpx[i] = mp[i]; qx[i] = q[i]; }
     diff[32] = 0; mpx[32] = 0; qx[32] = 0;
     st::sub(diff, diff, mpx, 33);
-    for (int it = 0; it < 3 && (diff[32] >> 31); it++) st::add(diff, diff, qx, 33);
+    for (int it = 0; it < 4 && (diff[32] >> 31); it++) st::add(diff, diff, qx, 33);
     while (diff[32] == 0 && st::cmp(diff, q, 32) >= 0) st::sub(diff, diff, qx, 33);
     uint32_t uu[32];
     st::mont_mul(uu, diff, A.k(KT_PINVQR, row), q, st::neg_inv32_st(q[0]), 32, scratch);
@@ -222,7 +223,8 @@ static __device__ __noinline__ void crt_combine(uint32_t* x128, const Arena& A, 
     for (int i = 0; i < 64; i++) { d[i] = yq[i]; ypr[i] = yp[i]; qx[i] = qq[i]; }
     d[64] = 0; ypr[64] = 0; qx[64] = 0;
     st::sub(d, d, ypr, 65);
-    for (int it = 0; it < 5 && (d[64] >> 31); it++) st::add(d, d, qx, 65);     // p^2 < 4 q^2: at most 4 additions
+    // p < 4q for every accepted key (see decrypt_finish), so yq - yp > -p^2 > -16 q^2: at most 16 additions
+    for (int it = 0; it < 16 && (d[64] >> 31); it++) st::add(d, d, qx, 65);
     uint32_t t[64];
     st::mont_mul(t, d, A.k(KT_PPINVQQR, row), qq, st::neg_inv32_st(qq[0]), 64, big);
     st::mul_add(x128, 128, t, 64, pp, 64, yp, 64);

@@ -8,9 +8,23 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 
 
 def load_keyset(index: int = 0):
-    """-> list of oracle.LocalKey for the 3 parties of key set `index`, plus the raw dict."""
+    """-> list of oracle.LocalKey for the 3 parties of key set `index`."""
     with open(os.path.join(HERE, "keys_t1n3.json")) as f:
-        ks = json.load(f)["keysets"][index]
+        return _local_keys(json.load(f)["keysets"][index])
+
+
+def edge_keysets_raw():
+    """the key sets of keys_edge.json as stored (hex strings, with each row's shape and p~, q~, xhi)"""
+    with open(os.path.join(HERE, "keys_edge.json")) as f:
+        return json.load(f)["keysets"]
+
+
+def load_edge_keysets():
+    """-> one list of oracle.LocalKey per key set of keys_edge.json (keys at the edges of the accepted domain)"""
+    return [_local_keys(ks) for ks in edge_keysets_raw()]
+
+
+def _local_keys(ks):
     parties = ks["parties"]
     eks, stmts, pks = [], [], []
     for p in parties:
