@@ -9,6 +9,8 @@ import pytest
 
 from oracle import blame_oracle as bo
 from oracle import gg20_oracle as o
+from tests.golden import fixtures
+from tests.test_edge_keys import _worst_plaintexts
 
 Q = o.Q
 
@@ -134,3 +136,46 @@ def test_blame_on_gpu_matches_oracle(engine, pkg, keyset):
     for name, phase, st, want in _corruptions(p5, p6, p7):
         assert run(phase, st) == _run_oracle(phase, st, R) == want, name
     ks.free()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("edge", [0, 1, 2], ids=lambda k: f"edge{k}")
+def test_blame_on_gpu_matches_oracle_on_edge_keysets(engine, pkg, edge):
+    """the same transcript and corruptions on each key set of keys_edge.json (2047-bit N, p < q, p/q close to 2 and to 4)"""
+    test_blame_on_gpu_matches_oracle(engine, pkg, fixtures.load_edge_keysets()[edge])
+
+
+@pytest.mark.gpu
+def test_paillier_open_on_edge_rows(engine):
+    """`Paillier::open` on every edge row: m = r = N - 1; c = N^2 - 1 (m = 0, r = N - 1); the plaintexts with (m mod p, m mod q) =
+    (p - 1, 0) and (0, q - 1), whose CRT tail needs the most corrections; and c + k N^2 < 2^4096 with its high 2048-bit half above N,
+    which a 2047-bit N allows: the job that computes r then reduces a high half larger than its modulus.  m and r equal the
+    oracle's, and (1 + m N) r^N = c mod N^2."""
+    from mpecdsa_b200 import blame, gg20
+    rows = [lk for ks in fixtures.load_edge_keysets() for lk in ks]
+    shapes = [r["shape"] for ks in fixtures.edge_keysets_raw() for r in ks["parties"]]
+    rng = random.Random(0x09E4)
+    idx, cs, kinds = [], [], []
+    for i, lk in enumerate(rows):
+        n = lk.dk.p * lk.dk.q
+        ek = o.EncryptionKey(n, n * n)
+        cases = [("m = r = N - 1", o.paillier_encrypt(ek, n - 1, n - 1)), ("N^2 - 1", ek.nn - 1)]
+        cases += [("worst residues", o.paillier_encrypt(ek, m, n - 1)) for m in _worst_plaintexts(lk.dk.p, lk.dk.q)]
+        c0 = o.paillier_encrypt(ek, rng.randrange(n), rng.randrange(1, n))
+        wide = c0 + ((1 << 4096) - 1 - c0) // ek.nn * ek.nn
+        assert wide >> 2048 > n or n.bit_length() == 2048, shapes[i]
+        if wide >> 2048 > n:
+            cases.append(("high half above N", wide))
+        for kind, c in cases:
+            idx.append(i); cs.append(c); kinds.append((shapes[i], kind))
+    assert sum(k == "high half above N" for _, k in kinds) >= 5
+    ks = gg20.KeySets(engine, fixtures.load_edge_keysets())
+    try:
+        m, r = blame.paillier_open(engine, ks, idx, cs)
+    finally:
+        ks.free()
+    want = [o.paillier_open(rows[i].dk, c) for i, c in zip(idx, cs)]
+    assert [kinds[j] for j in range(len(cs)) if (m[j], r[j]) != want[j]] == []
+    for i, c, mm, rr in zip(idx, cs, m, r):
+        n = rows[i].dk.p * rows[i].dk.q
+        assert (1 + mm * n) * pow(rr, n, n * n) % (n * n) == c % (n * n)

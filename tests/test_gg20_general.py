@@ -184,3 +184,46 @@ def test_general_signing_sets_on_gpu_match_oracle(engine, pkg):
     for p, wv in enumerate(want):
         assert int(out["status"][p]) == 0 and (out["R"][p], out["sigma"][p], out["k"][p], out["T"][p]) == (wv.R, wv.sigma_i, wv.k_i, wv.t_vec[p])
     ks5.free()
+
+
+@pytest.mark.gpu
+def test_general_signing_sets_on_edge_keys_match_oracle(engine):
+    """The size-generic driver over keys_edge.json.  One batch holds a three-signer session on each edge key set, so 2047- and
+    2048-bit moduli sit side by side and ciphertext and plaintext widths differ between the rows of every call; then a (t = 2, n = 5)
+    key over edge rows 0..4, signed by three of them with both rows whose p/q is close to 4.  Every output equals the oracle's."""
+    from mpecdsa_b200 import gg20, gg20_general
+    from tests.golden import fixtures
+    edge = fixtures.load_edge_keysets()
+    ks = gg20.KeySets(engine, edge)
+    rng = random.Random(0x6E2E)
+    sessions, owner = [], {}
+    for kidx, s_l in ((0, [2, 3, 1]), (1, [1, 2, 3]), (2, [3, 1, 2])):
+        keys, rnd = _session(rng, edge[kidx], s_l)
+        sessions.append((keys, s_l, rnd))
+        owner.update({id(lk): kidx for lk in keys})
+    try:
+        out = gg20_general.offline_batch(engine, ks, *_flatten(sessions, lambda lk, j: 3 * owner[id(lk)] + j))
+    finally:
+        ks.free()
+    u = 0
+    for keys, s_l, rnd in sessions:
+        want = gen.offline_session(keys, s_l, rnd)
+        assert _signature_ok(want, keys[0].y_sum_s, rng)
+        for p, wv in enumerate(want):
+            assert int(out["status"][u]) == wv.status == 0
+            assert (out["R"][u], out["sigma"][u], out["k"][u], out["T"][u]) == (wv.R, wv.sigma_i, wv.k_i, wv.t_vec[p]), (s_l, p)
+            u += 1
+    key5 = _five_party_key(edge, rng)
+    s_l = [5, 1, 3]                                   # edge rows 4 (q/p ~ 4), 0 (p/q ~ 4) and 2 (N just below 2^2048)
+    assert [(lk.dk.p * lk.dk.q).bit_length() for lk in (key5[i - 1] for i in s_l)] == [2047, 2047, 2048]
+    keys = [key5[i - 1] for i in s_l]
+    rnd = [_party_randomness(rng, lk, [s_l[gen._ind(p, j)] - 1 for j in range(2)]) for p, lk in enumerate(keys)]
+    want = gen.offline_session(keys, s_l, rnd)
+    assert [x.status for x in want] == [0, 0, 0] and _signature_ok(want, key5[0].y_sum_s, rng)
+    ks5 = gg20.KeySets(engine, edge)
+    try:
+        out = gg20_general.offline_batch(engine, ks5, *_flatten([(keys, s_l, rnd)], lambda lk, j: j))
+    finally:
+        ks5.free()
+    for p, wv in enumerate(want):
+        assert int(out["status"][p]) == 0 and (out["R"][p], out["sigma"][p], out["k"][p], out["T"][p]) == (wv.R, wv.sigma_i, wv.k_i, wv.t_vec[p])

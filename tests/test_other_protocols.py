@@ -1,7 +1,8 @@
 """Other protocols on the same primitives (SURVEY.md section 8(f) rank 4): Lindell-2017 two-party ECDSA, the interactive PDL proof and
 the GG18 phases 4 / 5a-5d.  CPU: the oracles' restatements run the reference's own test flows (`test_two_party_sign`,
 `test_full_key_gen` of lindell_2017/test.rs, the phase-5 part of gg_2018/test.rs `sign`) and the final signatures verify under an
-independent ECDSA (`cryptography`).  GPU: every new entry point against the oracle, bit for bit, plus tampered inputs."""
+independent ECDSA (`cryptography`).  GPU: every new entry point against the oracle, bit for bit, plus tampered inputs, on the
+standard key set and on the key sets of keys_edge.json, whose rows also carry inputs at the top of each sampling range."""
 import random
 
 import numpy as np
@@ -9,9 +10,19 @@ import pytest
 
 from oracle import gg18_oracle as e18
 from oracle import gg20_oracle as o
+from oracle import keygen_oracle as kg
 from oracle import lindell17_oracle as l17
+from tests.golden import fixtures
+from tests.golden.make_edge_keys import HALF, SLACK, prime_in
+from tests.test_edge_keys import _worst_plaintexts
 
 Q, G = o.Q, o.G
+
+
+def _edge_rows():
+    """(global key row, oracle.LocalKey, shape) of the 9 edge rows, in the order gg20.KeySets(engine, edge) uploads them"""
+    shapes = [r["shape"] for ks in fixtures.edge_keysets_raw() for r in ks["parties"]]
+    return [(i, lk, s) for i, (lk, s) in enumerate(zip([lk for ks in fixtures.load_edge_keysets() for lk in ks], shapes))]
 
 
 def _ecdsa_ok(r, s, pub, msg_int):
@@ -748,3 +759,163 @@ def test_lindell17_bulk_parity_on_gpu(engine, pkg, keyset):
         assert (r[i], s[i], int(rec[i])) == l17.p1_sign(c["dks"][i], want_c3, c["k1"][i], R2[i]), i
     assert all(_ecdsa_ok(r[i], s[i], c["pub"][i], c["msg"][i]) for i in range(0, n, 16))
     ks.free()
+
+
+# ------------------------------------------------------------------------------------------------ the same tests on the edge key sets
+@pytest.fixture(scope="module")
+def edge_keysets():
+    return fixtures.load_edge_keysets()
+
+
+# _l17_case puts party one on row i % 3, so every one of the 9 edge rows is party one in some run of these tests
+@pytest.mark.parametrize("edge", [0, 1, 2], ids=lambda k: f"edge{k}")
+@pytest.mark.parametrize("test", [test_lindell17_kernels_on_host_harness, test_zk_pdl_kernels_on_host_harness], ids=lambda f: f.__name__)
+def test_host_harness_on_edge_keysets(hh, edge_keysets, test, edge):
+    """the Lindell-2017 and zk-PDL host-harness tests on each key set of keys_edge.json (2047-bit N, p < q, p/q close to 2
+    and to 4, N at both ends of the accepted range)"""
+    test(hh, edge_keysets[edge])
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("edge", [0, 1, 2], ids=lambda k: f"edge{k}")
+@pytest.mark.parametrize("test", [test_lindell17_on_gpu_matches_oracle, test_zk_pdl_on_gpu_matches_oracle, test_gg18_whole_signing_on_gpu,
+                                  test_lindell17_full_key_gen_on_gpu, test_gg18_key_generation_then_signing_on_gpu,
+                                  test_lindell17_bulk_parity_on_gpu], ids=lambda f: f.__name__)
+def test_protocols_on_gpu_on_edge_keysets(engine, pkg, edge_keysets, test, edge):
+    """the GPU protocol tests above on each key set of keys_edge.json: decrypt_dev (p1_sign, the zk-PDL prover), GG18's index
+    bookkeeping over rows whose ciphertext and plaintext widths differ, and Lindell's key generation over 2047-bit N"""
+    test(engine, pkg, edge_keysets[edge])
+
+
+# ------------------------------------------------------------------------------------------------ edge key rows at the range tops
+def test_l17_case_puts_party_one_on_every_edge_row():
+    rows = {(lk.dk.p, lk.dk.q) for _, lk, _ in _edge_rows()}
+    used = {(d.p, d.q) for ks in fixtures.load_edge_keysets() for d in _l17_case(ks, random.Random(0), 3)["dks"]}
+    assert used == rows and len(rows) == 9
+    assert any(p / q > 3.9 for p, q in used) and any(q / p > 3.9 for p, q in used) and sum(p < q for p, q in used) >= 3
+
+
+def _wide_rho(p, q, base, rng, tries=256):
+    """rho above q^2 with base + rho q < N, drawn `tries` times, keeping the draw whose plaintext m = base + rho q has the largest
+    (m mod p) - (m mod q): the difference decrypt_finish has to bring into [0, q)"""
+    m = lambda r: base + r * Q
+    return max((rng.randrange(Q * Q, (p * q - base) // Q) for _ in range(tries)), key=lambda r: m(r) % p - m(r) % q)
+
+
+@pytest.mark.gpu
+def test_lindell17_range_tops_on_edge_rows(engine, pkg):
+    """Every edge row as party one's key, with each value at the top of its sampling range: rho = q^2 - 1, x1 = floor(q/3) - 1,
+    r_key = r_enc = N - 1, x2 = k1 = k2 = q - 1 (so k2^-1 = q - 1 as well) and the message 2^256 - 1.
+
+    Honest plaintexts stay below q^3, under both Paillier primes, so the CRT tail of p1_sign's decrypt has nothing to correct.  So
+    each row also gets a c3 from a party two whose rho lies above q^2: `PartialSig::compute` does not bound it, the signature is
+    the same because rho q vanishes mod q, and rho is picked so that (m mod p) - (m mod q) is large (more than 3 q on the rows with
+    p/q close to 4, where the tail needs its fourth addition of q)."""
+    from mpecdsa_b200 import gg20, lindell17 as L
+    rows = _edge_rows()
+    rng = random.Random(0x17ED)
+    x1, x2, k, msg, rho = Q // 3 - 1, Q - 1, Q - 1, (1 << 256) - 1, Q * Q - 1
+    R = o.pt_mul(G, k)                                                     # k1 = k2: both ephemeral public shares
+    pub = o.pt_mul(G, x1 * x2 % Q)
+    eks = [o.EncryptionKey(lk.dk.p * lk.dk.q, (lk.dk.p * lk.dk.q) ** 2) for _, lk, _ in rows]
+    n_list = [ek.n for ek in eks]
+    c_key = [o.paillier_encrypt(ek, x1, ek.n - 1) for ek in eks]
+    m = len(rows)
+    c3, st = L.p2_partial_sig(engine, n_list, list(range(m)), c_key, [x2] * m, [k] * m, [R] * m, [msg] * m, [rho] * m, [n - 1 for n in n_list])
+    assert not st.any()
+    assert c3 == [l17.p2_partial_sig(ek, ck, x2, k, R, msg, rho, ek.n - 1) for ek, ck in zip(eks, c_key)]
+    kinv = pow(k, -1, Q)
+    base = x1 * (kinv * (o.pt_mul(R, k)[0] % Q * x2 % Q) % Q) + kinv * msg % Q   # x1 v + (k2^-1 m mod q)
+    plain = [base + rho * Q] * m
+    for (_, lk, shape), ek, ck in zip(rows, eks, c_key):
+        p, q = lk.dk.p, lk.dk.q
+        r_w = _wide_rho(p, q, base, rng)
+        plain.append(base + r_w * Q)
+        assert plain[-1] < ek.n and (p < 3 * q or plain[-1] % p - plain[-1] % q > 3 * q), shape
+        c3.append(l17.p2_partial_sig(ek, ck, x2, k, R, msg, r_w, ek.n - 1))
+    key_row = list(range(m)) * 2
+    dks = [rows[i][1].dk for i in key_row]
+    assert [o.paillier_decrypt(d, c) for d, c in zip(dks, c3)] == plain
+    edge = fixtures.load_edge_keysets()
+    ks = gg20.KeySets(engine, edge)
+    try:
+        r, s, rec, st = L.p1_sign(engine, ks, key_row, c3, [k] * 2 * m, [R] * 2 * m)
+    finally:
+        ks.free()
+    want = [l17.p1_sign(d, c, k, R) for d, c in zip(dks, c3)]
+    wrong = [(rows[i][2], j >= m) for j, i in enumerate(key_row) if (r[j], s[j], int(rec[j])) != want[j]]
+    assert not st.any() and wrong == []
+    assert all(l17.verify(r[j], s[j], pub, msg) for j in range(2 * m)) and _ecdsa_ok(r[0], s[0], pub, msg)
+    assert not L.verify(engine, r, s, [pub] * 2 * m, [msg] * 2 * m).any()
+
+
+@pytest.mark.gpu
+def test_zk_pdl_range_tops_on_edge_rows(engine, pkg):
+    """Every edge row through the four messages with a = q - 1 and b = q^2 - 1, so that a + (b << bit_length(a)) has its largest
+    width, x1 = floor(q/3) - 1 and r = N - 1.  alpha = a x1 + b < q^3 again leaves the prover's CRT tail nothing to correct, so the
+    prover also decrypts the c' of a verifier that did not follow message1: the plaintexts with (m mod p, m mod q) = (p - 1, 0) and
+    (0, q - 1), the most the tail ever corrects (four additions of q on the rows with p/q close to 4)."""
+    from mpecdsa_b200 import gg20, lindell17 as L
+    rows = _edge_rows()
+    m = len(rows)
+    x1, a, b, blind = Q // 3 - 1, Q - 1, Q * Q - 1, Q - 1
+    assert (a + (b << a.bit_length())).bit_length() == 768
+    eks = [o.EncryptionKey(lk.dk.p * lk.dk.q, (lk.dk.p * lk.dk.q) ** 2) for _, lk, _ in rows]
+    n_list = [ek.n for ek in eks]
+    c_key = [o.paillier_encrypt(ek, x1, ek.n - 1) for ek in eks]
+    Qpt = o.pt_mul(G, x1)
+    ct, ctt, qt, st = L.pdl_verifier_message1(engine, n_list, list(range(m)), c_key, [Qpt] * m, [a] * m, [b] * m, [n - 1 for n in n_list], [blind] * m)
+    want = [l17.pdl_verifier_message1(ek, ck, Qpt, a, b, ek.n - 1, blind) for ek, ck in zip(eks, c_key)]
+    assert not st.any() and ct == [w.c_tag for w in want] and ctt == [w.c_tag_tag for w in want] and qt == [w.q_tag for w in want]
+    key_row, c_tag, plain = list(range(m)), list(ct), [a * x1 + b] * m
+    for i, (_, lk, _) in enumerate(rows):
+        for pl in _worst_plaintexts(lk.dk.p, lk.dk.q):
+            key_row.append(i); c_tag.append(o.paillier_encrypt(eks[i], pl, eks[i].n - 1)); plain.append(pl)
+    edge = fixtures.load_edge_keysets()
+    ks = gg20.KeySets(engine, edge)
+    try:
+        ch, qh, al, st = L.pdl_prover_message1(engine, ks, key_row, c_tag, [blind] * len(c_tag))
+    finally:
+        ks.free()
+    want_p = [l17.pdl_prover_message1(rows[i][1].dk, c, blind) for i, c in zip(key_row, c_tag)]
+    assert [w[2] for w in want_p] == plain
+    wrong = [(rows[i][2], j >= m) for j, i in enumerate(key_row) if (ch[j], qh[j], al[j]) != want_p[j]]
+    assert not st.any() and wrong == []
+    assert list(L.pdl_prover_message2(engine, [x1] * m, al[:m], ctt, [a] * m, [b] * m, [blind] * m)) == [0] * m
+    assert list(L.pdl_verifier_finalize(engine, ch[:m], qh[:m], [blind] * m, qt)) == [0] * m
+
+
+@pytest.mark.gpu
+def test_lindell17_paillier_key_size_rule(engine, pkg):
+    """Party two's `verify_ni_proof_correct_key` refuses `ek.n.bit_length() < PAILLIER_KEY_SIZE - 1` before it looks at the proof
+    (party_two.rs:307): party one's 2047-bit moduli pass p2_verify_paillier_and_proofs, and a 2046-bit N whose NiCorrectKeyProof
+    is valid gets IncorrectProof."""
+    from mpecdsa_b200 import gg20, keygen, lindell17 as L
+    edge = fixtures.load_edge_keysets()[0]
+    raw = fixtures.edge_keysets_raw()[0]["parties"]
+    rng = random.Random(0x2046)
+    small = (prime_in(HALF, HALF + SLACK, rng), prime_in(HALF >> 1, (HALF >> 1) + SLACK, rng))
+    # elements 0 and 1: rows 0 and 1 of edge key set 0; element 2 hands in the 2046-bit key (its PDL proof runs under row 2's key,
+    # which does not matter: the size rule decides first)
+    p_q = [(edge[i].dk.p, edge[i].dk.q) for i in range(2)] + [small]
+    n_list = [p * q for p, q in p_q]
+    assert [n.bit_length() for n in n_list] == [2047, 2047, 2046]
+    stm = [(edge[i].h1_h2_n_tilde_vec[i].N, edge[i].h1_h2_n_tilde_vec[i].g, edge[i].h1_h2_n_tilde_vec[i].ni) for i in range(3)]
+    # the CompositeDLogProof of (N~, h1, h2) is for the negated exponent phi(N~) - xhi (see keygen_oracle.h1_h2_n_tilde)
+    H = lambda r, k: int(r[k], 16)
+    neg_xhi = [(H(r, "p_tilde") - 1) * (H(r, "q_tilde") - 1) - H(r, "xhi") for r in raw]
+    x1 = [Q // 3 - 1] + [rng.randrange(1, Q // 3) for _ in range(2)]
+    pdl_rand = ([rng.randrange(Q ** 3) for _ in range(3)], [rng.randrange(1, n) for n in n_list], [rng.randrange(Q * s[0]) for s in stm],
+                [rng.randrange(Q ** 3 * s[0]) for s in stm])
+    ks = gg20.KeySets(engine, [edge])
+    try:
+        msg = L.p1_paillier_and_proofs(engine, ks, [0, 1, 2], [0, 1, 2], stm, neg_xhi, x1, [n - 1 for n in n_list], pdl_rand,
+                                       [rng.getrandbits(500) for _ in range(3)], p_q)
+        assert msg["correct_key_proof"] == [kg.correct_key_proof(o.DecryptionKey(p, q)) for p, q in p_q]
+        assert all(kg.correct_key_verify(sv, o.EncryptionKey(n, n * n)) for sv, n in zip(msg["correct_key_proof"], n_list))
+        assert list(keygen.correct_key_verify(engine, n_list, msg["correct_key_proof"])) == [0, 0, 0]
+        assert all(kg.composite_dlog_verify(kg.CompositeDLogProof(*pf), o.DLogStatement(*s_)) for pf, s_ in zip(msg["composite_dlog_proof"], stm))
+        st = L.p2_verify_paillier_and_proofs(engine, ks, [0, 1, 2], [0, 1, 2], stm, n_list, msg, msg["Q"])
+    finally:
+        ks.free()
+    assert list(st) == [0, 0, pkg.ST_PROOF]
