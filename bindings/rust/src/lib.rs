@@ -299,6 +299,27 @@ pub mod batch {
         Ok(rec)
     }
 
+    /// The sampling half of `MessageA::a`, `MessageB::b`, `AliceProof::generate`, `PDLwSlackProof::prove` and `SignKeys::create`
+    /// for a batch of sessions, drawn on the device from one 32-byte seed (`tecdsa_gg20_sample_randomness`): the `rnd` that
+    /// `offline_records` takes and one status byte per unit (0, or `TECDSA_ST_SAMPLING`).  Unit `2 s + position` has element id
+    /// `first_unit + 2 s + position`; a (seed, element id) pair must NEVER be used twice — a fresh seed from the OS CSPRNG per
+    /// call, or one seed with disjoint `first_unit` ranges.
+    pub fn sample_randomness(e: &Engine, ks: &KeySets, sessions: &[[u32; 3]], seed: &[u8; 32], first_unit: u64) -> Result<(Vec<u32>, Vec<u8>), EngineError> {
+        let n = sessions.len();
+        let flat: Vec<u32> = sessions.iter().flat_map(|s| s.iter().copied()).collect();
+        let mut words = [0u32; 8];
+        for (w, c) in words.iter_mut().zip(seed.chunks_exact(4)) {
+            *w = u32::from_le_bytes([c[0], c[1], c[2], c[3]]);
+        }
+        let mut rnd = vec![0u32; 2 * n * ffi::TECDSA_RND_LIMBS];
+        let mut status = vec![0u8; 2 * n];
+        let rc = unsafe { ffi::tecdsa_gg20_sample_randomness(e.raw(), ks.raw(), flat.as_ptr(), n, words.as_ptr(), first_unit, rnd.as_mut_ptr(), status.as_mut_ptr(), ffi::TECDSA_HOST) };
+        words = [0u32; 8];
+        let _ = words;
+        check(rc)?;
+        Ok((rnd, status))
+    }
+
     /// `party_two::PartialSig::compute` for a batch (two_party_ecdsa/lindell_2017/party_two.rs:390-424) with `rho` (< q^2) and the
     /// randomness of `Paillier::encrypt` explicit: c3 per element, or `None` where the reference would panic (k2 = 0).
     /// `n[key_idx[i]]` is the Paillier modulus of element i.

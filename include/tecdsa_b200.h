@@ -21,8 +21,10 @@
  *     aborts the batch and never panics, unlike the reference's assert!/unwrap() sites.
  *   - Calls are asynchronous on the context's stream for TECDSA_DEVICE, synchronous for
  *     TECDSA_HOST.  A context is not thread-safe; distinct contexts are independent.
- *   - No randomness is drawn inside the library: every sampled value of the reference
- *     (`BigInt::sample_below`, `Scalar::random`) is an explicit input.
+ *   - No call draws randomness on its own: every sampled value of the reference
+ *     (`BigInt::sample_below`, `Scalar::random`) is an explicit input.  The seeded sampler at the
+ *     end of this header (tecdsa_sample_batch, tecdsa_gg20_sample_randomness) produces those inputs
+ *     on the device from a 32-byte seed the caller draws from its OS CSPRNG.
  */
 #ifndef TECDSA_B200_H
 #define TECDSA_B200_H
@@ -55,7 +57,8 @@ enum {
     TECDSA_ST_INVALID_SIG = 9,    /* Error::InvalidSig           gg_2020/party_i.rs:908,934 */
     TECDSA_ST_PROOF = 10,         /* a curv sigma proof (DLog/Pedersen/HomoElGamal) failed to verify */
     TECDSA_ST_COMMITMENT = 11,    /* "bad gamma_i decommit"      gg_2020/party_i.rs:650-674 */
-    TECDSA_ST_INVALID_SS = 12     /* Error::InvalidSS            gg_2018/party_i.rs:262-281 (reported by the host-composed key-generation drivers) */
+    TECDSA_ST_INVALID_SS = 12,    /* Error::InvalidSS            gg_2018/party_i.rs:262-281 (reported by the host-composed key-generation drivers) */
+    TECDSA_ST_SAMPLING = 13       /* the seeded sampler: a bound no value can be drawn under, or TECDSA_SAMPLE_ATTEMPTS candidates rejected */
 };
 
 /* ---- context ------------------------------------------------------------------------ */
@@ -459,6 +462,57 @@ int tecdsa_gg20_offline_records(tecdsa_ctx* ctx, const tecdsa_keyset* ks, void* 
 int tecdsa_gg20_sign_batch(tecdsa_ctx* ctx, const tecdsa_keyset* ks, const uint32_t* sessions, size_t n_sessions, const uint32_t* message,
                            const uint32_t* R, const uint32_t* sigma, const uint32_t* k, uint32_t* s_i, uint32_t* sig_r, uint32_t* sig_s,
                            uint8_t* recid, uint8_t* status, int mem);
+/* ---- seeded sampling: the reference's `BigInt::sample_below`, `BigInt::sample`, `Scalar::random`, `sample_range` and
+ * `SampleFromMultiplicativeGroup` on the device ------------------------------------------------------------------------------
+ * The caller supplies one 32-byte seed (8 words, always read from HOST memory whatever `mem` says; it is staged in device
+ * scratch that is wiped before the call returns, like every staged secret) drawn from its OS CSPRNG.  Every value is a pure
+ * function of (seed, stream id, element id, bound): it does not depend on the batch it was drawn in, on thread scheduling or
+ * on the GPU, and a CPU restatement reproduces it bit for bit.
+ *
+ * THE ONE HARD RULE: a (seed, stream id, element id) triple must never be used twice.  Reuse repeats the values drawn under
+ * it; a repeated nonce k_i leaks the key share.  Use a fresh seed per call, or one seed with disjoint element-id ranges (that
+ * is how one logical batch is sharded over GPUs: rank g passes first_unit = 2 * the index of its first session).
+ *
+ * Generator: the ChaCha20 block function of RFC 8439 section 2.3 (20 rounds; state words 4..11 = seed, word 12 = block counter
+ * from 0, word 13 = stream id, words 14 | 15 = low | high half of the element id).  One attempt at a value of b bits consumes
+ * ceil(b / 512) whole 64-byte blocks: the first ceil(b / 32) keystream words are the little-endian limbs, the top limb is masked
+ * to b mod 32 bits, the rest of the last block is discarded.  Kinds:
+ *   TECDSA_SAMPLE_BITS    one attempt at `bits` bits, no rejection           `BigInt::sample(bits)`     gg_2020/party_i.rs:574
+ *   TECDSA_SAMPLE_BELOW   attempts at bit_length(bound) bits until < bound   `BigInt::sample_below`     mta/mod.rs:57,97-98
+ *   TECDSA_SAMPLE_UNIT    BELOW until gcd(v, bound) = 1     `SampleFromMultiplicativeGroup`     mta/range_proofs.rs:538-557
+ *   TECDSA_SAMPLE_RANGE1  1 + BELOW(bound - 2)              `sample_range(1, bound - 1)`      zk_pdl_with_slack/mod.rs:74
+ *   TECDSA_SAMPLE_SCALAR  BELOW(q) until non-zero           `Scalar::random()`                gg_2020/party_i.rs:563,565,628
+ * (uniform by rejection, never by modular reduction).  Only the distributions are the reference's; its OS RNG is not reproduced.
+ * An element whose TECDSA_SAMPLE_ATTEMPTS-th candidate is still rejected, or whose bound admits no value (bound = 0; bound = 1
+ * for UNIT; bound < 3 for RANGE1; a bound index >= n_bound), gets status TECDSA_ST_SAMPLING and an all-zero value.            */
+enum { TECDSA_SAMPLE_BITS = 0, TECDSA_SAMPLE_BELOW = 1, TECDSA_SAMPLE_UNIT = 2, TECDSA_SAMPLE_RANGE1 = 3, TECDSA_SAMPLE_SCALAR = 4 };
+enum { TECDSA_SAMPLE_ATTEMPTS = 256, TECDSA_SAMPLE_MAX_LIMBS = 128 };
+/* out[i] ([count][limbs], 1 <= limbs <= 128) = one value of `kind` for element id first_id + i on stream `stream`.  bound =
+ * [n_bound][limbs] (kinds BELOW, UNIT, RANGE1; element i uses row bound_idx[i], or row i when bound_idx == NULL); bits = the
+ * width of TECDSA_SAMPLE_BITS, 1 <= bits <= 32 * limbs; TECDSA_SAMPLE_SCALAR needs limbs >= 8.  A bad kind, width, limbs or mem
+ * and a null seed / out / status / required bound are TECDSA_E_ARG before anything is touched.                                */
+int tecdsa_sample_batch(tecdsa_ctx* ctx, const uint32_t seed[8], uint64_t first_id, uint32_t stream, int kind, int bits, const uint32_t* bound,
+                        const uint32_t* bound_idx, size_t n_bound, int limbs, uint32_t* out, uint8_t* status, size_t count, int mem);
+/* Stream ids of the fields of one offline unit's randomness record, in order of use.  The three range-proof statements of
+ * `MessageA::a` are folded into the id (TECDSA_RNDS_ALICE + 4 * statement + {0 alpha, 1 beta, 2 gamma, 3 rho}); nothing else is. */
+enum {
+    TECDSA_RNDS_GAMMA = 0, TECDSA_RNDS_K = 1, TECDSA_RNDS_BLIND = 2, TECDSA_RNDS_RK = 3, TECDSA_RNDS_ALICE = 4,
+    TECDSA_RNDS_BETATAG_GAMMA = 16, TECDSA_RNDS_R_GAMMA = 17, TECDSA_RNDS_NONCE_GAMMA_B = 18, TECDSA_RNDS_NONCE_GAMMA_BETA = 19,
+    TECDSA_RNDS_BETATAG_W = 20, TECDSA_RNDS_R_W = 21, TECDSA_RNDS_NONCE_W_B = 22, TECDSA_RNDS_NONCE_W_BETA = 23,
+    TECDSA_RNDS_L = 24, TECDSA_RNDS_PED_S1 = 25, TECDSA_RNDS_PED_S2 = 26,
+    TECDSA_RNDS_PDL_ALPHA = 27, TECDSA_RNDS_PDL_BETA = 28, TECDSA_RNDS_PDL_RHO = 29, TECDSA_RNDS_PDL_GAMMA = 30,
+    TECDSA_RNDS_HEG_S1 = 31, TECDSA_RNDS_HEG_S2 = 32, TECDSA_RNDS_COUNT = 33
+};
+/* rnd = [2*n_sessions][TECDSA_RND_LIMBS], the record tecdsa_gg20_offline_batch reads, every field drawn as the reference draws
+ * it: scalars SCALAR, the blind BITS(256), r_k BELOW(N_own), per statement x alpha BELOW(q^3), beta UNIT(N_own), gamma
+ * BELOW(q^3 N~_x), rho BELOW(q N~_x); beta', r' BELOW(N_peer); the PDL proof's alpha BELOW(q^3), beta RANGE1(N_own), rho
+ * BELOW(q N~_peer), gamma BELOW(q^3 N~_peer) — bounds from the uploaded key set.  Unit 2s + position of sessions[s] has element
+ * id first_unit + 2s + position; sessions as for tecdsa_gg20_offline_batch.  status[2*n_sessions]: TECDSA_ST_OK, or
+ * TECDSA_ST_SAMPLING for a unit whose descriptor names no key row or two equal parties (all-zero record) or one of whose fields
+ * ran out of attempts (that field zero).  With TECDSA_DEVICE the record never exists in host memory: this call, the offline
+ * batch and tecdsa_gg20_pack_records run back to back on device buffers.                                                  */
+int tecdsa_gg20_sample_randomness(tecdsa_ctx* ctx, const tecdsa_keyset* ks, const uint32_t* sessions, size_t n_sessions, const uint32_t seed[8],
+                                  uint64_t first_unit, uint32_t* rnd, uint8_t* status, int mem);
 /* 32x32+64 multiply-accumulates executed by the big-integer kernels of this context since creation / the last reset:
  * counted by the kernels themselves (one atomic add per job, from the loop trip counts of the products it ran) — the
  * "ops actually executed" figure of SURVEY.md section 8(d).  EC / hashing glue and the shift-subtract inversions are not

@@ -26,6 +26,8 @@ LIB_PATH = os.environ.get("TECDSA_B200_LIB") or os.path.join(_HERE, "libtecdsa_b
 HOST, DEVICE = 0, 1
 ST_OK, ST_EVEN_MODULUS, ST_INVALID_KEY, ST_RANGE, ST_NOT_INVERTIBLE, ST_HASH_MISMATCH = 0, 1, 2, 3, 4, 5
 ST_PDL_VERIFY, ST_PHASE5_BAD_SUM, ST_PHASE6, ST_INVALID_SIG, ST_PROOF, ST_COMMITMENT, ST_INVALID_SS = 6, 7, 8, 9, 10, 11, 12
+ST_SAMPLING = 13
+SAMPLE_BITS, SAMPLE_BELOW, SAMPLE_UNIT, SAMPLE_RANGE1, SAMPLE_SCALAR = 0, 1, 2, 3, 4      # TECDSA_SAMPLE_*
 
 # every symbol include/tecdsa_b200.h declares (checked by tests/test_abi.py)
 EXPORTS = [
@@ -51,6 +53,7 @@ EXPORTS = [
     "tecdsa_zkpdl_verifier_finalize_batch",
     "tecdsa_gg18_phase4_batch", "tecdsa_gg18_local_sig_batch", "tecdsa_gg18_phase5a_batch", "tecdsa_gg18_phase5c_batch", "tecdsa_gg18_phase5d_batch",
     "tecdsa_gg18_output_signature_batch",
+    "tecdsa_sample_batch", "tecdsa_gg20_sample_randomness",
 ]
 
 
@@ -469,6 +472,41 @@ def _sha256(self, messages):
     return [bytes(r) for r in out]
 
 
+def seed_words(seed: bytes) -> np.ndarray:
+    """a 32-byte seed as the 8 little-endian words the ABI takes"""
+    if len(seed) != 32:
+        raise ValueError("the sampler's seed is 32 bytes")
+    return np.frombuffer(bytes(seed), dtype="<u4").copy()
+
+
+def _sample(self, kind: int, count: int, seed: bytes, stream: int = 0, first_id: int = 0, bound=None, bound_idx=None, bits: int = 0,
+            limbs: Optional[int] = None):
+    """Batched seeded sampling (tecdsa_sample_batch): element i = one value of `kind` (SAMPLE_*) on `stream` for element id
+    first_id + i.  bound = list of ints, one per element, or a table that bound_idx[i] indexes.  -> (values, status); a value whose
+    status is ST_SAMPLING is 0.  A (seed, stream, element id) triple must never be used twice."""
+    lib = self.lib
+    if not getattr(lib, "_sample_bound", False):
+        V, S, I = ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int
+        lib.tecdsa_sample_batch.argtypes = [V, V, ctypes.c_uint64, ctypes.c_uint32, I, I, V, V, S, I, V, V, S, I]
+        lib._sample_bound = True
+    bounded = kind in (SAMPLE_BELOW, SAMPLE_UNIT, SAMPLE_RANGE1)
+    if limbs is None:
+        width = 256 if kind == SAMPLE_SCALAR else bits if kind == SAMPLE_BITS else max([int(b).bit_length() for b in bound] + [1])
+        limbs = (width + 127) // 128 * 4
+    B = ints_to_limbs(bound, limbs) if bounded else None
+    idx = None if bound_idx is None or not bounded else np.asarray(bound_idx, dtype=np.uint32)
+    out = np.zeros((count, limbs), dtype=np.uint32)
+    st = np.full(count, 255, dtype=np.uint8)
+    sw = seed_words(seed)
+    try:
+        self._ck(lib.tecdsa_sample_batch(self._ctx, _ptr(sw), first_id, stream, kind, bits, _ptr(B), _ptr(idx), 0 if B is None else B.shape[0], limbs,
+                                         _ptr(out), _ptr(st), count, HOST), "sample_batch")
+    finally:
+        sw[:] = 0
+    return limbs_to_ints(out), st
+
+
+Engine.sample = _sample
 Engine.point_add, Engine.point_compress, Engine.point_decompress, Engine.scalar_op = _point_add, _point_compress, _point_decompress, _scalar_op
 Engine.scalar_from_bigint, Engine.wide_muladd, Engine.unit_mod_check, Engine.sha256 = _scalar_from_bigint, _wide_muladd, _unit_mod_check, _sha256
 Engine.mod_mul, Engine.mod_inv, Engine.secp_mul = _mod_mul, _mod_inv, _secp_mul

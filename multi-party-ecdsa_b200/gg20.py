@@ -5,11 +5,12 @@ calls tecdsa_gg20_offline_batch.  No arithmetic happens here."""
 from __future__ import annotations
 
 import ctypes
-from typing import List, Sequence
+import os
+from typing import List, Optional, Sequence
 
 import numpy as np
 
-from . import HOST, Engine, EngineError, ints_to_limbs, limbs_to_ints, _ptr
+from . import HOST, Engine, EngineError, ints_to_limbs, limbs_to_ints, seed_words, _ptr
 
 RND_LIMBS = 1408
 # (offset, limbs) of every field of the randomness record — include/tecdsa_b200.h TECDSA_RND_*
@@ -144,6 +145,47 @@ def sign_batch(eng: Engine, keys: KeySets, sessions: np.ndarray, message: np.nda
     eng._ck(lib.tecdsa_gg20_sign_batch(eng._ctx, keys.handle, _ptr(sessions), n, *[_ptr(x) for x in ins], _ptr(s_i), _ptr(r), _ptr(s), _ptr(recid), _ptr(status), HOST),
             "gg20_sign_batch")
     return {"s_i": s_i, "r": r, "s": s, "recid": recid, "status": status}
+
+
+# TECDSA_RNDS_*: the sampler's stream id of every field of the randomness record (Alice fields: RNDS_ALICE + 4 * statement + part)
+RNDS = {"gamma": 0, "k": 1, "blind": 2, "r_k": 3, "beta_tag_gamma": 16, "r_gamma": 17, "nonce_gamma_b": 18, "nonce_gamma_beta": 19,
+        "beta_tag_w": 20, "r_w": 21, "nonce_w_b": 22, "nonce_w_beta": 23, "l": 24, "ped_s1": 25, "ped_s2": 26,
+        "pdl_alpha": 27, "pdl_beta": 28, "pdl_rho": 29, "pdl_gamma": 30, "heg_s1": 31, "heg_s2": 32}
+RNDS_ALICE = 4
+
+
+def fresh_seed(seed: Optional[bytes] = None) -> bytes:
+    """The caller's 32-byte seed, or a fresh one from the OS CSPRNG — the one place the product touches it.  A seed drawn here is
+    used for the one call it was drawn for and is never returned to the caller, stored or logged."""
+    return os.urandom(32) if seed is None else bytes(seed)
+
+
+def sample_randomness(eng: Engine, keys: KeySets, sessions, seed: Optional[bytes] = None, first_unit: int = 0, mem: int = HOST, rnd=None, status=None):
+    """The sampling half of the reference's `MessageA::a`, `MessageB::b`, `AliceProof::generate`, `PDLwSlackProof::prove`,
+    `SignKeys::create` for a batch of sessions (tecdsa_gg20_sample_randomness): -> (rnd [2n][RND_LIMBS], status [2n]), the record
+    `offline_batch` takes, every field a function of (seed, first_unit + unit, field, key material).  seed=None draws a fresh one.
+    A (seed, unit id) pair must never be used twice: fresh seed per call, or one seed with disjoint first_unit ranges.
+    mem=DEVICE: sessions, rnd and status are the caller's CUDA tensors and the record never reaches the host."""
+    _bind(eng.lib)
+    lib = eng.lib
+    if not getattr(lib, "_gg20_sample_bound", False):
+        V = ctypes.c_void_p
+        lib.tecdsa_gg20_sample_randomness.argtypes = [V, V, V, ctypes.c_size_t, V, ctypes.c_uint64, V, V, ctypes.c_int]
+        lib._gg20_sample_bound = True
+    if mem == HOST:
+        sessions = np.ascontiguousarray(np.asarray(sessions, dtype=np.uint32).reshape(-1, 3))
+        n = sessions.shape[0]
+        rnd = np.zeros((2 * n, RND_LIMBS), dtype=np.uint32)
+        status = np.full(2 * n, 255, dtype=np.uint8)
+    else:
+        n = sessions.shape[0]
+    sw = seed_words(fresh_seed(seed))
+    try:
+        eng._ck(lib.tecdsa_gg20_sample_randomness(eng._ctx, keys.handle, _ptr(sessions), n, _ptr(sw), first_unit, _ptr(rnd), _ptr(status), mem),
+                "gg20_sample_randomness")
+    finally:
+        sw[:] = 0
+    return rnd, status
 
 
 def debug_field(eng: Engine, name: str, units: int) -> np.ndarray:

@@ -6,11 +6,11 @@ instances.  Element u = session * ttag + position; pair t = u * (ttag - 1) + j i
 No arithmetic happens on the host — only index bookkeeping and equality tests.  Oracle: oracle/gg20_general_oracle.py."""
 from __future__ import annotations
 
-from typing import Dict, List, Sequence
+from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 
-from . import Engine, limbs_to_ints
+from . import SAMPLE_BELOW, SAMPLE_BITS, SAMPLE_RANGE1, SAMPLE_SCALAR, SAMPLE_UNIT, Engine, EngineError, limbs_to_ints
 from . import gg18, gg20
 from .gg20 import KeySets, unpack_point
 
@@ -19,6 +19,52 @@ ST_INVALID_KEY, ST_PDL, ST_PHASE5, ST_PHASE6, ST_PROOF, ST_COMMIT = 2, 6, 7, 8, 
 
 def _pts_of(a: np.ndarray):
     return [unpack_point(v) for v in limbs_to_ints(a)]
+
+
+def sample_rnd(eng: Engine, keys: KeySets, ttag: int, key_rows: Sequence[int], all_rows: Sequence[Sequence[int]], seed: Optional[bytes] = None) -> Dict[str, list]:
+    """The `rnd` dictionary `offline_batch` takes, every value drawn on the device as the reference draws it inside `MessageA::a`,
+    `MessageB::b`, `AliceProof::generate`, `PDLwSlackProof::prove` and `SignKeys::create` (ranges: oracle/sampling.py::sample_unit),
+    one `Engine.sample` call per field.  Streams are the TECDSA_RNDS_* ids of the fused call's record (`gg20.RNDS`; the Alice fields
+    use RNDS_ALICE + part for every statement).  Element id = (sub << 32) | u for element u = session * ttag + position, with sub =
+    0 for the per-element fields, the statement index x for alice[u][x], and the peer index j for the per-pair fields of pair
+    u * (ttag - 1) + j — so no (stream, id) repeats inside a call.  seed=None draws a fresh seed; a seed serves ONE call."""
+    seed = gg20.fresh_seed(seed)
+    U, P1 = len(key_rows), ttag - 1
+    q = gg20._Q
+    N, NT = keys.table(0, 64), keys.table(2, 64)
+    peer_row = [[key_rows[u // ttag * ttag + (j if j < u % ttag else j + 1)] for u in range(U)] for j in range(P1)]
+
+    def draw(kind, name, sub=0, bound=None, bits=0, limbs=None, stream=None):
+        vals, st = eng.sample(kind, U, seed, stream=gg20.RNDS[name] if stream is None else stream, first_id=sub << 32, bound=bound, bits=bits, limbs=limbs)
+        if st.any():
+            raise EngineError(f"sampling {name}: element {int(np.flatnonzero(st)[0])} has status {int(st[st != 0][0])}")
+        return vals
+
+    rnd = {f: draw(SAMPLE_SCALAR, f) for f in ("gamma", "k", "l", "ped_s1", "ped_s2", "heg_s1", "heg_s2")}
+    rnd["blind"] = draw(SAMPLE_BITS, "blind", bits=256)
+    n_own = [N[r] for r in key_rows]
+    rnd["r_k"] = draw(SAMPLE_BELOW, "r_k", bound=n_own)
+    n_st = len(all_rows[0]) if U else 0
+    per_st = []
+    for x in range(n_st):
+        nt = [NT[all_rows[u][x]] for u in range(U)]
+        A = gg20.RNDS_ALICE
+        per_st.append((draw(SAMPLE_BELOW, "alice alpha", x, [q ** 3] * U, stream=A), draw(SAMPLE_UNIT, "alice beta", x, n_own, stream=A + 1),
+                       draw(SAMPLE_BELOW, "alice gamma", x, [q ** 3 * v for v in nt], stream=A + 2), draw(SAMPLE_BELOW, "alice rho", x, [q * v for v in nt], stream=A + 3)))
+    rnd["alice"] = [[tuple(part[u] for part in per_st[x]) for x in range(n_st)] for u in range(U)]
+    per_pair = {f: [None] * (U * P1) for f in ("beta_tag_gamma", "r_gamma", "nonce_gamma_b", "nonce_gamma_beta", "beta_tag_w", "r_w", "nonce_w_b", "nonce_w_beta", "pdl")}
+    for j in range(P1):
+        n_peer, nt_peer = [N[r] for r in peer_row[j]], [NT[r] for r in peer_row[j]]
+        cols = {f: draw(SAMPLE_BELOW, f, j, n_peer) for f in ("beta_tag_gamma", "r_gamma", "beta_tag_w", "r_w")}
+        cols.update({f: draw(SAMPLE_SCALAR, f, j) for f in ("nonce_gamma_b", "nonce_gamma_beta", "nonce_w_b", "nonce_w_beta")})
+        pdl = (draw(SAMPLE_BELOW, "pdl_alpha", j, [q ** 3] * U), draw(SAMPLE_RANGE1, "pdl_beta", j, n_own), draw(SAMPLE_BELOW, "pdl_rho", j, [q * v for v in nt_peer]),
+               draw(SAMPLE_BELOW, "pdl_gamma", j, [q ** 3 * v for v in nt_peer]))
+        for u in range(U):
+            for f, col in cols.items():
+                per_pair[f][u * P1 + j] = col[u]
+            per_pair["pdl"][u * P1 + j] = tuple(p[u] for p in pdl)
+    rnd.update(per_pair)
+    return rnd
 
 
 def offline_batch(eng: Engine, keys: KeySets, ttag: int, key_rows: Sequence[int], all_rows: Sequence[Sequence[int]], w: Sequence[int],
