@@ -114,7 +114,8 @@ int tecdsa_secp_mul_batch(tecdsa_ctx* ctx, const uint32_t* points, const uint32_
  * secp_scalar_{mul,add,sub,inv}: `Scalar * + - invert()` (party_i.rs:599-617,635-640,857-863); inv: ok = 0 for zero.
  * secp_scalar_from_bigint: `Scalar::from(&BigInt)` — a `limbs`-limb integer reduced mod q (mta/mod.rs:132,166).
  * wide_muladd: a*b + c over the integers, no modulus (`e * a + alpha`, `e * rho + gamma`; mta/range_proofs.rs:87-88):
- *   out_limbs >= a_limbs + b_limbs and > c_limbs.
+ *   exact for every operand value, so out_limbs >= max(a_limbs + b_limbs, c_limbs) + 1, or out_limbs == a_limbs + b_limbs
+ *   with c_limbs <= max(a_limbs, b_limbs); other widths are refused with TECDSA_E_ARG.
  * unit_mod_check: the acceptance test of `SampleFromMultiplicativeGroup::from_modulo / from_paillier_key`
  *   (mta/range_proofs.rs:538-557): ok = 1 iff r < N and gcd(r, N) = 1 (odd N; mod_bits 2048 or 4096) — the caller's sampling
  *   loop draws again where ok = 0, exactly as the reference's `while r.gcd(N) != 1`.

@@ -442,7 +442,9 @@ def _scalar_from_bigint(self, x, limbs=64):
 
 
 def _wide_muladd(self, a, b, c, a_limbs, b_limbs, c_limbs, out_limbs):
-    """Batched exact a*b + c (no modulus)"""
+    """Batched exact a*b + c (no modulus).  out_limbs must hold the result for every operand value: out_limbs >=
+    max(a_limbs + b_limbs, c_limbs) + 1, or out_limbs == a_limbs + b_limbs with c_limbs <= max(a_limbs, b_limbs); other
+    widths raise EngineError (TECDSA_E_ARG)."""
     _bind_ec(self.lib)
     A, B, C = ints_to_limbs(a, a_limbs), ints_to_limbs(b, b_limbs), ints_to_limbs(c, c_limbs)
     out = np.zeros((len(a), out_limbs), dtype=np.uint32)

@@ -169,10 +169,18 @@ extern "C" int tecdsa_secp_scalar_from_bigint_batch(tecdsa_ctx* c, const uint32_
     KCHECK();
     return S.finish();
 }
+// The widths must make a*b + c fit in out_limbs for EVERY operand value (st::mul_add drops a carry out of the top limb):
+// one limb above both a*b and c, or exactly a_limbs + b_limbs when c is no wider than the wider factor
+// ((2^(32A) - 1)(2^(32B) - 1) + 2^(32 max(A,B)) - 1 < 2^(32(A+B))).
+static bool wide_muladd_fits(int a_limbs, int b_limbs, int c_limbs, int out_limbs) {
+    const int ab = a_limbs + b_limbs, wider = a_limbs > b_limbs ? a_limbs : b_limbs;
+    return out_limbs >= (ab > c_limbs ? ab : c_limbs) + 1 || (out_limbs == ab && c_limbs <= wider);
+}
 extern "C" int tecdsa_wide_muladd_batch(tecdsa_ctx* c, const uint32_t* a, int a_limbs, const uint32_t* b, int b_limbs, const uint32_t* addend, int c_limbs,
                                         uint32_t* out, int out_limbs, size_t count, int mem) {
-    if (!a || !b || !addend || !out || a_limbs <= 0 || b_limbs <= 0 || c_limbs <= 0 || out_limbs < a_limbs + b_limbs || out_limbs < c_limbs + 1 || out_limbs > 512)
-        return tecdsa_fail(TECDSA_E_ARG, "wide_muladd: bad argument");
+    if (!a || !b || !addend || !out || a_limbs <= 0 || b_limbs <= 0 || c_limbs <= 0 || out_limbs > 512 ||
+        !wide_muladd_fits(a_limbs, b_limbs, c_limbs, out_limbs))
+        return tecdsa_fail(TECDSA_E_ARG, "wide_muladd: bad argument (out_limbs must hold a*b + c for all operand values)");
     STAGE_PROLOGUE("wide_muladd", count);
     const uint32_t *da = S.in(a, count * (size_t)a_limbs), *db = S.in(b, count * (size_t)b_limbs), *dc = S.in(addend, count * (size_t)c_limbs);
     uint32_t* dout = S.out(out, count * (size_t)out_limbs);
