@@ -251,6 +251,50 @@ int tecdsa_vss_share_batch(tecdsa_ctx* ctx, int t, int n_shares, const uint32_t*
 int tecdsa_h1_h2_n_tilde_batch(tecdsa_ctx* ctx, const uint32_t* p_t, const uint32_t* q_t, const uint32_t* h1, const uint32_t* xhi,
                                uint32_t* n_tilde, uint32_t* h2, uint32_t* xhi_neg, uint32_t* xhi_inv_neg, uint8_t* status, size_t count, int mem);
 
+/* ---- GG20 key generation as one call: `Keygen` Round0..Round4 (gg_2020/state_machine/keygen/rounds.rs:26-300) ---------------
+ * `groups` independent groups of n parties; element e = g*n + (i-1) is party i of group g; E = groups*n.  Limits 1 <= t <= n-1
+ * (state_machine/keygen.rs:57-61) and 2 <= n <= 64, else TECDSA_E_ARG.  Every value the reference samples inside `Keys::create`,
+ * `phase1_broadcast_phase3_proof_of_correct_key_proof_of_correct_h1h2`, `VerifiableSS::share` and `DLogProof::prove` is an input
+ * (the seeded sampler draws them: TECDSA_RNDS_KG_* below); primes are inputs.  Every pointer of both structs is required and
+ * lives where `mem` says.  Outputs are the fields of `LocalKey` (keygen/rounds.rs:310-322): a group's paillier_key_vec and
+ * h1_h2_n_tilde_vec are its members' `n` and `dlog_st` rows in order.
+ * Status per element = the error its own `proceed` returns, rounds in order; a group stops at the first round in which any member
+ * failed (complete[g] = 0, its LocalKey outputs zero; members that did not fail keep TECDSA_ST_OK):
+ *   TECDSA_ST_NOT_INVERTIBLE  that element's xhi has no inverse mod phi(N~), a draw the reference repeats (party_i.rs:144-149);
+ *   TECDSA_ST_INVALID_KEY     every element, when a sender's commitment does not reopen, its NiCorrectKeyProof or either
+ *                             CompositeDLogProof fails, or N or N~ is outside 2047..2048 bits (party_i.rs:266-320);
+ *   TECDSA_ST_INVALID_SS      a receiver for which a sender's share fails `validate_share` or commitments[0] != y_j (:322-367);
+ *   TECDSA_ST_PROOF           every element, when a sender's DLogProof fails or pk != commitments_to_xi[j] (:405-438).
+ * bad_actors[e] = bit j for party j+1 in that element's `ErrorType.bad_actors`.
+ * Declared work-saving identity, value-preserving: every receiver runs the same deterministic checks on the same broadcast and the
+ * same DLogProof, so each is verified once per sender, not n times; the n^2 share validations run per (receiver, sender) pair.
+ * Every intermediate (coefficients, shares, x_i, xhi, phi, N^-1 mod phi) lives in stage scratch wiped before the call returns.    */
+typedef struct {
+    const uint32_t* paillier_p;   /* [E][32]     Paillier prime p (`Paillier::keypair`, party_i.rs:162)                       */
+    const uint32_t* paillier_q;   /* [E][32]     Paillier prime q                                                            */
+    const uint32_t* n_tilde_p;    /* [E][32]     N~ prime p~ (`generate_h1_h2_N_tilde`, party_i.rs:137-156)                   */
+    const uint32_t* n_tilde_q;    /* [E][32]     N~ prime q~                                                                 */
+    const uint32_t* u;            /* [E][8]      u_i = the polynomial's coefficient 0 (`Keys::create`)                       */
+    const uint32_t* coeffs;       /* [E][t][8]   a_1..a_t (`VerifiableSS::share`, party_i.rs:313)                           */
+    const uint32_t* blind;        /* [E][8]      commitment blind (`BigInt::sample(256)`, party_i.rs:222)                   */
+    const uint32_t* h1;           /* [E][64]     h1 < N~                                                                     */
+    const uint32_t* xhi;          /* [E][64]     xhi < phi(N~)                                                               */
+    const uint32_t* cdl_nonce;    /* [E][2][16]  the nonces r of the CompositeDLogProofs of bases h1 and h2 (< 2^512)        */
+    const uint32_t* dlog_nonce;   /* [E][8]      the nonce of DLogProof::prove(x_i)                                         */
+} tecdsa_keygen_in;
+typedef struct {
+    uint32_t* x_i;                /* [E][8]        keys_linear.x_i                                                           */
+    uint32_t* vss;                /* [E][t+1][16]  vss_scheme.commitments of the element's own polynomial                    */
+    uint32_t* n;                  /* [E][64]       its Paillier N (paillier_key_vec row)                                     */
+    uint32_t* dlog_st;            /* [E][3][64]    its (N~, h1, h2) (h1_h2_n_tilde_vec row)                                  */
+    uint32_t* y;                  /* [groups][16]  y_sum_s                                                                   */
+    uint32_t* pk;                 /* [groups][n][16] pk_vec                                                                  */
+    uint8_t* status;              /* [E]                                                                                      */
+    uint64_t* bad_actors;         /* [E]                                                                                      */
+    uint8_t* complete;            /* [groups]      1 = every member holds its LocalKey                                       */
+} tecdsa_keygen_out;
+int tecdsa_gg20_keygen_batch(tecdsa_ctx* ctx, int t, int n, size_t groups, int mem, const tecdsa_keygen_in* in, const tecdsa_keygen_out* out);
+
 /* ---- identifiable abort (SURVEY.md section 8(f) rank 3; gg_2020/blame.rs) ------------------------------------------------
  * paillier_open: `Paillier::open(dk, c)` (blame.rs:252-256) over an uploaded key set: m = Dec(c) [count][64] and the
  *   randomness r [count][64] with c = (1 + m N) r^N mod N^2 (r = (c mod N)^(N^-1 mod phi(N)) mod N).
@@ -503,6 +547,15 @@ enum {
     TECDSA_RNDS_L = 24, TECDSA_RNDS_PED_S1 = 25, TECDSA_RNDS_PED_S2 = 26,
     TECDSA_RNDS_PDL_ALPHA = 27, TECDSA_RNDS_PDL_BETA = 28, TECDSA_RNDS_PDL_RHO = 29, TECDSA_RNDS_PDL_GAMMA = 30,
     TECDSA_RNDS_HEG_S1 = 31, TECDSA_RNDS_HEG_S2 = 32, TECDSA_RNDS_COUNT = 33
+};
+/* Stream ids of the inputs of the GG20 key-generation call, disjoint from the offline record's.  Element id = (sub << 32) | e
+ * for element e of the batch (plus the caller's first id): sub = 0 for the per-element values, k - 1 for coefficient a_k, and 0 / 1
+ * for the CompositeDLog nonces of bases h1 / h2.  Kinds as the reference draws them: u_i, a_k and the DLog nonce SCALAR; blind
+ * BITS(256); h1 BELOW(N~); xhi UNIT(phi(N~)) (`sample_below(phi)` until `mod_inv` exists, party_i.rs:144-149); the
+ * CompositeDLog nonces BITS(512) (zk-paillier [R]).                                                                            */
+enum {
+    TECDSA_RNDS_KG_U = 64, TECDSA_RNDS_KG_COEFF = 65, TECDSA_RNDS_KG_BLIND = 66, TECDSA_RNDS_KG_H1 = 67, TECDSA_RNDS_KG_XHI = 68,
+    TECDSA_RNDS_KG_CDL = 69, TECDSA_RNDS_KG_DLOG = 70
 };
 /* rnd = [2*n_sessions][TECDSA_RND_LIMBS], the record tecdsa_gg20_offline_batch reads, every field drawn as the reference draws
  * it: scalars SCALAR, the blind BITS(256), r_k BELOW(N_own), per statement x alpha BELOW(q^3), beta UNIT(N_own), gamma

@@ -5,8 +5,11 @@
 #include "stage.cuh"
 #include "primorial.h"
 #include "even_inverse.cuh"
+#include "keygen_kernels.cuh"
 
 using namespace tecdsa;
+
+#include <climits>
 
 int tecdsa_internal_fb_points_set_keygen(const uint32_t* table) {
     CK(cudaMemcpyToSymbol(secp::g_fb_points, &table, sizeof(table)));
@@ -133,32 +136,14 @@ __global__ void k_cd_post(const uint32_t* v, const uint32_t* x, const uint8_t* p
 __global__ void k_vss_validate(const uint32_t* commitments, int n_comm, const uint32_t* share, const uint32_t* index, uint8_t* status, int count) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= count) return;
-    const uint32_t* C = commitments + (size_t)i * n_comm * 16;
-    U256 idx = u256_zero();
-    idx.v[0] = index[i];
-    bool ok = n_comm > 0;
-    Jac acc = jac_identity();
-    for (int j = n_comm - 1; j >= 0 && ok; j--) {
-        Affine cj = affine_load(C + (size_t)j * 16);
-        if (!cj.inf && !on_curve(cj)) { ok = false; break; }
-        if (j != n_comm - 1) acc = jac_mul(acc, idx);
-        acc = jac_add(acc, jac_from_affine(cj));
-    }
-    Affine lhs = mul_G(sc_from_limbs(share + (size_t)i * 8, 8));
-    status[i] = (ok && affine_eq(lhs, jac_to_affine(acc))) ? TECDSA_ST_OK : TECDSA_ST_PROOF;
+    status[i] = kg::vss_share_ok(commitments + (size_t)i * n_comm * 16, n_comm, share + (size_t)i * 8, index[i]) ? TECDSA_ST_OK : TECDSA_ST_PROOF;
 }
 
-}  // namespace
 
-extern "C" int tecdsa_correct_key_verify_batch(tecdsa_ctx* c, const uint32_t* n_mod, const uint32_t* sigma, const uint8_t* salt, int salt_len,
-                                               uint8_t* status, size_t count, int mem) {
-    if (!n_mod || !sigma || !status || salt_len < 0 || salt_len > 64 || (salt_len && !salt)) return tecdsa_fail(TECDSA_E_ARG, "correct_key_verify: bad argument");
-    STAGE_PROLOGUE("correct_key_verify", count);
-    const int n = (int)count;
+// NiCorrectKeyProof::verify on staged device buffers: n = [count][64], sigma = [count][11][64] -> status
+int correct_key_verify_step(tecdsa_ctx* c, Stage& S, int n, const uint32_t* dn, const uint32_t* ds, const uint8_t* dsalt, int salt_len, uint8_t* dst) {
+    const size_t count = (size_t)n;
     const int tot = n * 11;
-    const uint32_t *dn = S.in(n_mod, count * 64), *ds = S.in(sigma, count * 11 * 64);
-    const uint8_t* dsalt = S.in(salt, (size_t)(salt_len ? salt_len : 0));
-    uint8_t* dst = S.out(status, count);
     uint32_t *rho72 = S.tmp<uint32_t>((size_t)tot * 72), *rho = S.tmp<uint32_t>((size_t)tot * 64), *got = S.tmp<uint32_t>((size_t)tot * 64);
     uint32_t *idx = S.tmp<uint32_t>(tot), *one = S.tmp<uint32_t>(4), *pmod = S.tmp<uint32_t>(count * 64), *pinv = S.tmp<uint32_t>(count * 64);
     uint8_t* gcd_ok = S.tmp<uint8_t>(count);
@@ -187,17 +172,13 @@ extern "C" int tecdsa_correct_key_verify_batch(tecdsa_ctx* c, const uint32_t* n_
     RUN(run(c, L.e64, 64));
     k_ck_cmp<<<grid_for(count), 64, 0, c->stream>>>(dn, got, rho, gcd_ok, dst, n);
     KCHECK();
-    return S.finish();
+    return 0;
 }
 
-extern "C" int tecdsa_composite_dlog_verify_batch(tecdsa_ctx* c, const uint32_t* n_tilde, const uint32_t* g, const uint32_t* ni, const uint32_t* x,
-                                                  const uint32_t* y, int y_limbs, uint8_t* status, size_t count, int mem) {
-    if (!n_tilde || !g || !ni || !x || !y || !status || y_limbs <= 0 || y_limbs > 128) return tecdsa_fail(TECDSA_E_ARG, "composite_dlog_verify: bad argument");
-    STAGE_PROLOGUE("composite_dlog_verify", count);
-    const int n = (int)count;
-    const uint32_t *dN = S.in(n_tilde, count * 64), *dg = S.in(g, count * 64), *dni = S.in(ni, count * 64), *dx = S.in(x, count * 64);
-    const uint32_t* dy = S.in(y, count * (size_t)y_limbs);
-    uint8_t* dst = S.out(status, count);
+// CompositeDLogProof::verify on staged device buffers
+int composite_dlog_verify_step(tecdsa_ctx* c, Stage& S, int n, const uint32_t* dN, const uint32_t* dg, const uint32_t* dni, const uint32_t* dx,
+                               const uint32_t* dy, int y_limbs, uint8_t* dst) {
+    const size_t count = (size_t)n;
     uint32_t *e8 = S.tmp<uint32_t>(count * 8), *v = S.tmp<uint32_t>(count * 64), *scratch = S.tmp<uint32_t>(count * 64 * 2);
     uint8_t *pre_ok = S.tmp<uint8_t>(count), *ok_g = S.tmp<uint8_t>(count), *ok_ni = S.tmp<uint8_t>(count);
     if (S.err) return S.err;
@@ -213,6 +194,32 @@ extern "C" int tecdsa_composite_dlog_verify_batch(tecdsa_ctx* c, const uint32_t*
     RUN(run(c, L.e64, 64));
     k_cd_post<<<grid_for(count), 64, 0, c->stream>>>(v, dx, pre_ok, ok_g, ok_ni, dst, n);
     KCHECK();
+    return 0;
+}
+
+}  // namespace
+
+extern "C" int tecdsa_correct_key_verify_batch(tecdsa_ctx* c, const uint32_t* n_mod, const uint32_t* sigma, const uint8_t* salt, int salt_len,
+                                               uint8_t* status, size_t count, int mem) {
+    if (!n_mod || !sigma || !status || salt_len < 0 || salt_len > 64 || (salt_len && !salt)) return tecdsa_fail(TECDSA_E_ARG, "correct_key_verify: bad argument");
+    STAGE_PROLOGUE("correct_key_verify", count);
+    const uint32_t *dn = S.in(n_mod, count * 64), *ds = S.in(sigma, count * 11 * 64);
+    const uint8_t* dsalt = S.in(salt, (size_t)(salt_len ? salt_len : 0));
+    uint8_t* dst = S.out(status, count);
+    if (S.err) return S.err;
+    RUN(correct_key_verify_step(c, S, (int)count, dn, ds, dsalt, salt_len, dst));
+    return S.finish();
+}
+
+extern "C" int tecdsa_composite_dlog_verify_batch(tecdsa_ctx* c, const uint32_t* n_tilde, const uint32_t* g, const uint32_t* ni, const uint32_t* x,
+                                                  const uint32_t* y, int y_limbs, uint8_t* status, size_t count, int mem) {
+    if (!n_tilde || !g || !ni || !x || !y || !status || y_limbs <= 0 || y_limbs > 128) return tecdsa_fail(TECDSA_E_ARG, "composite_dlog_verify: bad argument");
+    STAGE_PROLOGUE("composite_dlog_verify", count);
+    const uint32_t *dN = S.in(n_tilde, count * 64), *dg = S.in(g, count * 64), *dni = S.in(ni, count * 64), *dx = S.in(x, count * 64);
+    const uint32_t* dy = S.in(y, count * (size_t)y_limbs);
+    uint8_t* dst = S.out(status, count);
+    if (S.err) return S.err;
+    RUN(composite_dlog_verify_step(c, S, (int)count, dN, dg, dni, dx, dy, y_limbs, dst));
     return S.finish();
 }
 
@@ -235,6 +242,11 @@ extern "C" int tecdsa_vss_validate_share_batch(tecdsa_ctx* c, const uint32_t* co
 // so the Kaliski job list (odd moduli only) serves `BigInt::mod_inv(&xhi, &phi)` (party_i.rs:146) and N^-1 mod phi(N)
 // (zk-paillier correct_key_ni.rs `proof` [R]).
 namespace {
+
+// zk-paillier `SALT_STRING` [R] ("KZen"): the salt of the NiCorrectKeyProof of key generation (party_i.rs:225,288-291)
+const uint8_t KEYGEN_SALT[4] = {75, 90, 101, 110};
+// CompositeDLogProof response width in key generation: y = r + e * (phi - xhi) < 2^512 + 2^2304 fits 73 limbs, rounded to 4
+constexpr int CDL_Y_LIMBS = 76;
 
 // CompositeDLogProof::prove tail (zk-paillier composite_dlog_proof.rs [R]; call sites party_i.rs:238-241):
 // e = H(x, g, N, ni), y = r + e * secret over the integers
@@ -277,21 +289,12 @@ __global__ void k_fill_u8(uint8_t* p, uint8_t v, int count) {
     if (i < count) p[i] = v;
 }
 
-}  // namespace
-
-// NiCorrectKeyProof::proof(&dk, None) (zk-paillier correct_key_ni.rs [R]; call site party_i.rs:225):
-// sigma_j = rho_j^(N^-1 mod phi(N)) mod N for j < 11.  p, q = [count][32]; sigma = [count][11][64].
-extern "C" int tecdsa_correct_key_prove_batch(tecdsa_ctx* c, const uint32_t* p, const uint32_t* q, const uint8_t* salt, int salt_len,
-                                              uint32_t* sigma, uint8_t* status, size_t count, int mem) {
-    if (!p || !q || !sigma || !status || salt_len < 0 || salt_len > 64 || (salt_len && !salt)) return tecdsa_fail(TECDSA_E_ARG, "correct_key_prove: bad argument");
-    STAGE_PROLOGUE("correct_key_prove", count);
-    const int n = (int)count;
+// NiCorrectKeyProof::proof(&dk, None) on staged device buffers; N = p*q is written to `N` [count][64]
+int correct_key_prove_step(tecdsa_ctx* c, Stage& S, int n, const uint32_t* dp, const uint32_t* dq, const uint8_t* dsalt, int salt_len, uint32_t* dsig,
+                           uint8_t* dst, uint32_t* N) {
+    const size_t count = (size_t)n;
     const int tot = n * 11;
-    const uint32_t *dp = S.in(p, count * 32), *dq = S.in(q, count * 32);
-    const uint8_t* dsalt = S.in(salt, (size_t)(salt_len ? salt_len : 0));
-    uint32_t* dsig = S.out(sigma, count * 11 * 64);
-    uint8_t* dst = S.out(status, count);
-    uint32_t *N = S.tmp<uint32_t>(count * 64), *phi = S.tmp<uint32_t>(count * 64), *phinv = S.tmp<uint32_t>(count * 64), *d = S.tmp<uint32_t>(count * 64);
+    uint32_t *phi = S.tmp<uint32_t>(count * 64), *phinv = S.tmp<uint32_t>(count * 64), *d = S.tmp<uint32_t>(count * 64);
     uint32_t *rho72 = S.tmp<uint32_t>((size_t)tot * 72), *rho = S.tmp<uint32_t>((size_t)tot * 64), *idx = S.tmp<uint32_t>(tot), *one = S.tmp<uint32_t>(4);
     uint8_t* ok = S.tmp<uint8_t>(count);
     if (S.err) return S.err;
@@ -315,55 +318,31 @@ extern "C" int tecdsa_correct_key_prove_batch(tecdsa_ctx* c, const uint32_t* p, 
     RUN(run(c, L.e64, 64));
     add_exp(L.e64, 64, tot, Nt, 1, arr(rho, 64), tab(d, idx, 64), 64, NONE, NONE, 0, 0, NONE, NONE, dsig, 64);
     RUN(run(c, L.e64, 64));
-    return S.finish();
+    return 0;
 }
 
-// CompositeDLogProof::prove(&DLogStatement{N, g, ni}, &secret) (party_i.rs:238-241): nonce r = [count][16] (< 2^512),
-// secret = [count][secret_limbs]; x = g^r mod N [count][64], y = r + e*secret [count][y_limbs], y_limbs >= secret_limbs + 9.
-extern "C" int tecdsa_composite_dlog_prove_batch(tecdsa_ctx* c, const uint32_t* n_tilde, const uint32_t* g, const uint32_t* ni, const uint32_t* secret,
-                                                 int secret_limbs, const uint32_t* r, uint32_t* x, uint32_t* y, int y_limbs, size_t count, int mem) {
-    if (!n_tilde || !g || !ni || !secret || !r || !x || !y || secret_limbs <= 0 || secret_limbs > 64 || y_limbs < secret_limbs + 9 || y_limbs > 128 || (y_limbs & 3))
-        return tecdsa_fail(TECDSA_E_ARG, "composite_dlog_prove: bad argument");
-    STAGE_PROLOGUE("composite_dlog_prove", count);
-    const int n = (int)count;
-    const uint32_t *dN = S.in(n_tilde, count * 64), *dg = S.in(g, count * 64), *dni = S.in(ni, count * 64);
-    const uint32_t *dsec = S.in(secret, count * (size_t)secret_limbs), *dr = S.in(r, count * 16);
-    uint32_t *dx = S.out(x, count * 64), *dy = S.out(y, count * (size_t)y_limbs);
-    if (S.err) return S.err;
+// CompositeDLogProof::prove on staged device buffers
+int composite_dlog_prove_step(tecdsa_ctx* c, int n, const uint32_t* dN, const uint32_t* dg, const uint32_t* dni, const uint32_t* dsec, int secret_limbs,
+                              const uint32_t* dr, uint32_t* dx, uint32_t* dy, int y_limbs) {
     Launches L;
     add_exp(L.e64, 64, n, arr(dN, 64), 1, arr(dg, 64), arr(dr, 16), 16, NONE, NONE, 0, 0, NONE, NONE, dx, 64);
     RUN(run(c, L.e64, 64));
-    k_cd_prove_post<<<grid_for(count), 64, 0, c->stream>>>(dN, dg, dni, dx, dsec, secret_limbs, dr, dy, y_limbs, n);
+    k_cd_prove_post<<<grid_for((size_t)n), 64, 0, c->stream>>>(dN, dg, dni, dx, dsec, secret_limbs, dr, dy, y_limbs, n);
     KCHECK();
-    return S.finish();
+    return 0;
 }
 
-// VerifiableSS::share(t, n, &secret) with explicit coefficients (party_i.rs:313): coefficients = [count][t+1][8] (index 0 = the
-// secret) -> shares [count][n][8] = f(1..n) mod q, commitments [count][t+1][16] = a_j * G.
-extern "C" int tecdsa_vss_share_batch(tecdsa_ctx* c, int t, int n_shares, const uint32_t* coefficients, uint32_t* shares, uint32_t* commitments,
-                                      size_t count, int mem) {
-    if (!coefficients || !shares || !commitments || t < 0 || t > 63 || n_shares <= 0 || n_shares > 4096) return tecdsa_fail(TECDSA_E_ARG, "vss_share: bad argument");
-    STAGE_PROLOGUE("vss_share", count);
-    const int t1 = t + 1;
-    const uint32_t* dc = S.in(coefficients, count * (size_t)t1 * 8);
-    uint32_t *dsh = S.out(shares, count * (size_t)n_shares * 8), *dcm = S.out(commitments, count * (size_t)t1 * 16);
-    if (S.err) return S.err;
-    k_vss_share<<<grid_for(count * (size_t)(t1 + n_shares)), 64, 0, c->stream>>>(dc, t1, n_shares, dsh, dcm, (int)count);
+// VerifiableSS::share on staged device buffers
+int vss_share_step(tecdsa_ctx* c, int n, int t1, int n_shares, const uint32_t* dc, uint32_t* dsh, uint32_t* dcm) {
+    k_vss_share<<<grid_for((size_t)n * (size_t)(t1 + n_shares)), 64, 0, c->stream>>>(dc, t1, n_shares, dsh, dcm, n);
     KCHECK();
-    return S.finish();
+    return 0;
 }
 
-// generate_h1_h2_N_tilde (party_i.rs:137-156) with its samples explicit: p~, q~ = [count][32] primes, h1 < N~, xhi < phi ->
-// N~ = p~ q~, h2 = h1^xhi mod N~, and the NEGATED exponents phi - xhi, phi - xhi^-1 the function returns.  status NOT_INVERTIBLE
-// where the reference's sampling loop would draw again (`mod_inv(&xhi, &phi)` is None, :146-149).
-extern "C" int tecdsa_h1_h2_n_tilde_batch(tecdsa_ctx* c, const uint32_t* p_t, const uint32_t* q_t, const uint32_t* h1, const uint32_t* xhi,
-                                          uint32_t* n_tilde, uint32_t* h2, uint32_t* xhi_neg, uint32_t* xhi_inv_neg, uint8_t* status, size_t count, int mem) {
-    if (!p_t || !q_t || !h1 || !xhi || !n_tilde || !h2 || !xhi_neg || !xhi_inv_neg || !status) return tecdsa_fail(TECDSA_E_ARG, "h1_h2_n_tilde: bad argument");
-    STAGE_PROLOGUE("h1_h2_n_tilde", count);
-    const int n = (int)count;
-    const uint32_t *dp = S.in(p_t, count * 32), *dq = S.in(q_t, count * 32), *dh1 = S.in(h1, count * 64), *dxhi = S.in(xhi, count * 64);
-    uint32_t *dN = S.out(n_tilde, count * 64), *dh2 = S.out(h2, count * 64), *dxn = S.out(xhi_neg, count * 64), *dxin = S.out(xhi_inv_neg, count * 64);
-    uint8_t* dst = S.out(status, count);
+// generate_h1_h2_N_tilde on staged device buffers
+int h1_h2_n_tilde_step(tecdsa_ctx* c, Stage& S, int n, const uint32_t* dp, const uint32_t* dq, const uint32_t* dh1, const uint32_t* dxhi, uint32_t* dN,
+                       uint32_t* dh2, uint32_t* dxn, uint32_t* dxin, uint8_t* dst) {
+    const size_t count = (size_t)n;
     uint32_t *phi = S.tmp<uint32_t>(count * 64), *minv = S.tmp<uint32_t>(count * 64);
     uint8_t* ok = S.tmp<uint8_t>(count);
     if (S.err) return S.err;
@@ -379,6 +358,146 @@ extern "C" int tecdsa_h1_h2_n_tilde_batch(tecdsa_ctx* c, const uint32_t* p_t, co
     k_inv_even_post<<<grid_for(count), 64, 0, c->stream>>>(dxhi, phi, minv, ok, dxin, 1, dst, n);   // phi - xhi^-1 mod phi
     KCHECK();
     k_lin_sub<<<grid_for(count), 64, 0, c->stream>>>(phi, dxhi, dxn, n);
+    KCHECK();
+    return 0;
+}
+
+}  // namespace
+
+// NiCorrectKeyProof::proof(&dk, None) (zk-paillier correct_key_ni.rs [R]; call site party_i.rs:225):
+// sigma_j = rho_j^(N^-1 mod phi(N)) mod N for j < 11.  p, q = [count][32]; sigma = [count][11][64].
+extern "C" int tecdsa_correct_key_prove_batch(tecdsa_ctx* c, const uint32_t* p, const uint32_t* q, const uint8_t* salt, int salt_len,
+                                              uint32_t* sigma, uint8_t* status, size_t count, int mem) {
+    if (!p || !q || !sigma || !status || salt_len < 0 || salt_len > 64 || (salt_len && !salt)) return tecdsa_fail(TECDSA_E_ARG, "correct_key_prove: bad argument");
+    STAGE_PROLOGUE("correct_key_prove", count);
+    const uint32_t *dp = S.in(p, count * 32), *dq = S.in(q, count * 32);
+    const uint8_t* dsalt = S.in(salt, (size_t)(salt_len ? salt_len : 0));
+    uint32_t* dsig = S.out(sigma, count * 11 * 64);
+    uint8_t* dst = S.out(status, count);
+    uint32_t* N = S.tmp<uint32_t>(count * 64);
+    if (S.err) return S.err;
+    RUN(correct_key_prove_step(c, S, (int)count, dp, dq, dsalt, salt_len, dsig, dst, N));
+    return S.finish();
+}
+
+// CompositeDLogProof::prove(&DLogStatement{N, g, ni}, &secret) (party_i.rs:238-241): nonce r = [count][16] (< 2^512),
+// secret = [count][secret_limbs]; x = g^r mod N [count][64], y = r + e*secret [count][y_limbs], y_limbs >= secret_limbs + 9.
+extern "C" int tecdsa_composite_dlog_prove_batch(tecdsa_ctx* c, const uint32_t* n_tilde, const uint32_t* g, const uint32_t* ni, const uint32_t* secret,
+                                                 int secret_limbs, const uint32_t* r, uint32_t* x, uint32_t* y, int y_limbs, size_t count, int mem) {
+    if (!n_tilde || !g || !ni || !secret || !r || !x || !y || secret_limbs <= 0 || secret_limbs > 64 || y_limbs < secret_limbs + 9 || y_limbs > 128 || (y_limbs & 3))
+        return tecdsa_fail(TECDSA_E_ARG, "composite_dlog_prove: bad argument");
+    STAGE_PROLOGUE("composite_dlog_prove", count);
+    const uint32_t *dN = S.in(n_tilde, count * 64), *dg = S.in(g, count * 64), *dni = S.in(ni, count * 64);
+    const uint32_t *dsec = S.in(secret, count * (size_t)secret_limbs), *dr = S.in(r, count * 16);
+    uint32_t *dx = S.out(x, count * 64), *dy = S.out(y, count * (size_t)y_limbs);
+    if (S.err) return S.err;
+    RUN(composite_dlog_prove_step(c, (int)count, dN, dg, dni, dsec, secret_limbs, dr, dx, dy, y_limbs));
+    return S.finish();
+}
+
+// VerifiableSS::share(t, n, &secret) with explicit coefficients (party_i.rs:313): coefficients = [count][t+1][8] (index 0 = the
+// secret) -> shares [count][n][8] = f(1..n) mod q, commitments [count][t+1][16] = a_j * G.
+extern "C" int tecdsa_vss_share_batch(tecdsa_ctx* c, int t, int n_shares, const uint32_t* coefficients, uint32_t* shares, uint32_t* commitments,
+                                      size_t count, int mem) {
+    if (!coefficients || !shares || !commitments || t < 0 || t > 63 || n_shares <= 0 || n_shares > 4096) return tecdsa_fail(TECDSA_E_ARG, "vss_share: bad argument");
+    STAGE_PROLOGUE("vss_share", count);
+    const int t1 = t + 1;
+    const uint32_t* dc = S.in(coefficients, count * (size_t)t1 * 8);
+    uint32_t *dsh = S.out(shares, count * (size_t)n_shares * 8), *dcm = S.out(commitments, count * (size_t)t1 * 16);
+    if (S.err) return S.err;
+    RUN(vss_share_step(c, (int)count, t1, n_shares, dc, dsh, dcm));
+    return S.finish();
+}
+
+// generate_h1_h2_N_tilde (party_i.rs:137-156) with its samples explicit: p~, q~ = [count][32] primes, h1 < N~, xhi < phi ->
+// N~ = p~ q~, h2 = h1^xhi mod N~, and the NEGATED exponents phi - xhi, phi - xhi^-1 the function returns.  status NOT_INVERTIBLE
+// where the reference's sampling loop would draw again (`mod_inv(&xhi, &phi)` is None, :146-149).
+extern "C" int tecdsa_h1_h2_n_tilde_batch(tecdsa_ctx* c, const uint32_t* p_t, const uint32_t* q_t, const uint32_t* h1, const uint32_t* xhi,
+                                          uint32_t* n_tilde, uint32_t* h2, uint32_t* xhi_neg, uint32_t* xhi_inv_neg, uint8_t* status, size_t count, int mem) {
+    if (!p_t || !q_t || !h1 || !xhi || !n_tilde || !h2 || !xhi_neg || !xhi_inv_neg || !status) return tecdsa_fail(TECDSA_E_ARG, "h1_h2_n_tilde: bad argument");
+    STAGE_PROLOGUE("h1_h2_n_tilde", count);
+    const uint32_t *dp = S.in(p_t, count * 32), *dq = S.in(q_t, count * 32), *dh1 = S.in(h1, count * 64), *dxhi = S.in(xhi, count * 64);
+    uint32_t *dN = S.out(n_tilde, count * 64), *dh2 = S.out(h2, count * 64), *dxn = S.out(xhi_neg, count * 64), *dxin = S.out(xhi_inv_neg, count * 64);
+    uint8_t* dst = S.out(status, count);
+    if (S.err) return S.err;
+    RUN(h1_h2_n_tilde_step(c, S, (int)count, dp, dq, dh1, dxhi, dN, dh2, dxn, dxin, dst));
+    return S.finish();
+}
+
+// ------------------------------------------------------------------------------------------ GG20 key generation, Round0..Round4
+// (state_machine/keygen/rounds.rs:26-300) for `groups` groups of n parties in one staged call; see the header for the layouts.
+// Every broadcast and every DLog proof is verified once per sender (every receiver runs the same deterministic check on the same
+// message); the n^2 share validations run per (receiver, sender) pair.  All intermediates live in stage scratch.
+extern "C" int tecdsa_gg20_keygen_batch(tecdsa_ctx* c, int t, int n, size_t groups, int mem, const tecdsa_keygen_in* in, const tecdsa_keygen_out* out) {
+    if (t < 1 || t > n - 1 || n < 2 || n > 64 || !in || !out || groups > (size_t)(INT_MAX / 64) / (11 * (size_t)n))
+        return tecdsa_fail(TECDSA_E_ARG, "gg20_keygen: bad argument");
+    if (!in->paillier_p || !in->paillier_q || !in->n_tilde_p || !in->n_tilde_q || !in->u || !in->coeffs || !in->blind || !in->h1 || !in->xhi ||
+        !in->cdl_nonce || !in->dlog_nonce || !out->x_i || !out->vss || !out->n || !out->dlog_st || !out->y || !out->pk || !out->status ||
+        !out->bad_actors || !out->complete)
+        return tecdsa_fail(TECDSA_E_ARG, "gg20_keygen: null buffer");
+    const size_t E = groups * (size_t)n;
+    STAGE_PROLOGUE("gg20_keygen", E);
+    const int e = (int)E, t1 = t + 1;
+    const size_t R = 64 * sizeof(uint32_t);                 // bytes of one 2048-bit row
+    const uint32_t *dp = S.in(in->paillier_p, E * 32), *dq = S.in(in->paillier_q, E * 32), *dpt = S.in(in->n_tilde_p, E * 32), *dqt = S.in(in->n_tilde_q, E * 32);
+    const uint32_t *du = S.in(in->u, E * 8), *da = S.in(in->coeffs, E * (size_t)t * 8), *dblind = S.in(in->blind, E * 8);
+    const uint32_t *dh1 = S.in(in->h1, E * 64), *dxhi = S.in(in->xhi, E * 64), *dcdl = S.in(in->cdl_nonce, E * 32), *ddl = S.in(in->dlog_nonce, E * 8);
+    uint32_t *ox = S.out(out->x_i, E * 8), *ovss = S.out(out->vss, E * (size_t)t1 * 16), *oN = S.out(out->n, E * 64), *ost = S.out(out->dlog_st, E * 3 * 64);
+    uint32_t *oy = S.out(out->y, groups * 16), *opk = S.out(out->pk, E * 16);
+    uint8_t *ostatus = S.out(out->status, E), *ocomplete = S.out(out->complete, groups);
+    uint64_t* obad = S.out(out->bad_actors, E);
+    // NT = [N~; N~], H = [h1; h2; h1] (statement 1 is (N~, h1, h2), statement 2 (N~, h2, h1)), SEC = [phi - xhi; phi - xhi^-1],
+    // RN = [r1; r2]: the two CompositeDLog proofs of every party run as one batch of 2E
+    uint32_t *NT = S.tmp<uint32_t>(2 * E * 64), *H = S.tmp<uint32_t>(3 * E * 64), *SEC = S.tmp<uint32_t>(2 * E * 64), *RN = S.tmp<uint32_t>(2 * E * 16);
+    uint32_t *X = S.tmp<uint32_t>(2 * E * 64), *Y = S.tmp<uint32_t>(2 * E * CDL_Y_LIMBS), *sigma = S.tmp<uint32_t>(E * 11 * 64);
+    uint32_t *coeff = S.tmp<uint32_t>(E * t1 * 8), *shares = S.tmp<uint32_t>(E * (size_t)n * 8), *com = S.tmp<uint32_t>(E * 8);
+    uint32_t *proof = S.tmp<uint32_t>(E * 40), *gcomm = S.tmp<uint32_t>(groups * (size_t)t1 * 16);
+    uint8_t *st_nt = S.tmp<uint8_t>(E), *st_ckp = S.tmp<uint8_t>(E), *st_ck = S.tmp<uint8_t>(E), *st_cd = S.tmp<uint8_t>(2 * E), *ok2 = S.tmp<uint8_t>(E);
+    uint8_t *pair_ok = S.tmp<uint8_t>(E * (size_t)n), *ok4 = S.tmp<uint8_t>(E), *salt = S.tmp<uint8_t>(sizeof(KEYGEN_SALT));
+    if (S.err) return S.err;
+    const cudaStream_t st = c->stream;
+    if (cudaMemcpyAsync(salt, KEYGEN_SALT, sizeof(KEYGEN_SALT), cudaMemcpyHostToDevice, st) != cudaSuccess ||
+        cudaMemcpyAsync(H, dh1, E * R, cudaMemcpyDeviceToDevice, st) != cudaSuccess ||
+        cudaMemcpyAsync(H + 2 * E * 64, dh1, E * R, cudaMemcpyDeviceToDevice, st) != cudaSuccess ||
+        cudaMemcpy2DAsync(RN, 16 * 4, dcdl, 32 * 4, 16 * 4, E, cudaMemcpyDeviceToDevice, st) != cudaSuccess ||
+        cudaMemcpy2DAsync(RN + E * 16, 16 * 4, dcdl + 16, 32 * 4, 16 * 4, E, cudaMemcpyDeviceToDevice, st) != cudaSuccess ||
+        cudaMemcpy2DAsync(coeff, t1 * 32, du, 32, 32, E, cudaMemcpyDeviceToDevice, st) != cudaSuccess ||
+        cudaMemcpy2DAsync(coeff + 8, t1 * 32, da, t * 32, t * 32, E, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+        return tecdsa_fail(TECDSA_E_CUDA, "gg20_keygen: copy");
+    // Round 0 / 1: Keys::create and phase1_broadcast_phase3_proof_of_correct_key_proof_of_correct_h1h2 (party_i.rs:137-258)
+    RUN(h1_h2_n_tilde_step(c, S, e, dpt, dqt, H, dxhi, NT, H + E * 64, SEC, SEC + E * 64, st_nt));
+    if (cudaMemcpyAsync(NT + E * 64, NT, E * R, cudaMemcpyDeviceToDevice, st) != cudaSuccess) return tecdsa_fail(TECDSA_E_CUDA, "gg20_keygen: copy");
+    // the prover's NOT_INVERTIBLE (no N^-1 mod phi) is not read: its exponent is then 0, every sigma is 1, and the
+    // Round-2 NiCorrectKeyProof verification rejects that sender, as the reference's verifiers would reject its broadcast
+    RUN(correct_key_prove_step(c, S, e, dp, dq, salt, (int)sizeof(KEYGEN_SALT), sigma, st_ckp, oN));
+    RUN(composite_dlog_prove_step(c, 2 * e, NT, H, H + E * 64, SEC, 64, RN, X, Y, CDL_Y_LIMBS));
+    RUN(vss_share_step(c, e, t1, n, coeff, shares, ovss));
+    kg::k_kg_commit<<<grid_for(E), 64, 0, st>>>(ovss, t1, dblind, com, e);
+    KCHECK();
+    // Round 2 (party_i.rs:266-320), once per sender.  Here the decommitted y_i IS the sender's commitment 0 (ovss row 0) and com was
+    // made above from the same y_i and blind, so the reopening check, like Round 3's commitments[0] == y_j, is a self-consistency
+    // check of this call: it cannot fail here, and it is kept so that the kernels run every check the reference runs
+    RUN(correct_key_verify_step(c, S, e, oN, sigma, salt, (int)sizeof(KEYGEN_SALT), st_ck));
+    RUN(composite_dlog_verify_step(c, S, 2 * e, NT, H, H + E * 64, X, Y, CDL_Y_LIMBS, st_cd));
+    kg::k_kg_round2<<<grid_for(E), 64, 0, st>>>(ovss, t1 * 16, dblind, com, st_ck, oN, NT, st_cd, ok2, e);
+    KCHECK();
+    // Round 3 (party_i.rs:322-367): every (receiver, sender) share, x_i, the DLog proof of x_i
+    kg::k_kg_validate_pairs<<<grid_for(E * n), 64, 0, st>>>(ovss, t1, ovss, t1 * 16, shares, n, pair_ok, e * n);
+    KCHECK();
+    kg::k_kg_xi<<<grid_for(E), 64, 0, st>>>(shares, n, ox, e);
+    KCHECK();
+    kg::k_kg_dlog_prove<<<grid_for(E), 64, 0, st>>>(ox, ddl, proof, e);
+    KCHECK();
+    // Round 4 (party_i.rs:369-438), once per sender
+    kg::k_kg_global_commitments<<<grid_for(groups * t1), 64, 0, st>>>(ovss, t1, n, gcomm, (int)groups);
+    KCHECK();
+    kg::k_kg_round4<<<grid_for(E), 64, 0, st>>>(gcomm, t1, n, proof, ok4, e);
+    KCHECK();
+    // LocalKey (keygen/rounds.rs:282-296): h1_h2_n_tilde_vec rows (N~, h1, h2), then status, masks, completion
+    for (int k = 0; k < 3; k++)
+        if (cudaMemcpy2DAsync(ost + k * 64, 3 * R, (k ? H + (k - 1) * E * 64 : NT), R, R, E, cudaMemcpyDeviceToDevice, st) != cudaSuccess)
+            return tecdsa_fail(TECDSA_E_CUDA, "gg20_keygen: copy");
+    kg::k_kg_finish<<<grid_for(E), 64, 0, st>>>(n, t1, st_nt, ok2, pair_ok, ok4, proof, gcomm, ostatus, obad, ocomplete, opk, oy, ox, ovss, oN, ost, e);
     KCHECK();
     return S.finish();
 }

@@ -195,19 +195,22 @@ def local_key(lk, commitments: Sequence[Point], enc: Encoding = DEFAULT) -> Dict
 
 
 @dataclass
-class _DK:
+class DecryptionKey:
+    """paillier `DecryptionKey` {p, q}"""
     p: int
     q: int
 
 
 @dataclass
-class _EK:
+class EncryptionKey:
+    """paillier `EncryptionKey` {n, nn}"""
     n: int
     nn: Optional[int] = None        # the engine derives N^2 on the device
 
 
 @dataclass
-class _ST:
+class DLogStatement:
+    """zk-paillier `DLogStatement` {N, g, ni} = (N~, h1, h2)"""
     N: int
     g: int
     ni: int
@@ -220,10 +223,10 @@ class LoadedLocalKey:
     t: int
     n: int
     x_i: int
-    dk: _DK
+    dk: DecryptionKey
     pk_vec: List[Point]
-    paillier_key_vec: List[_EK]
-    h1_h2_n_tilde_vec: List[_ST]
+    paillier_key_vec: List[EncryptionKey]
+    h1_h2_n_tilde_vec: List[DLogStatement]
     y_sum_s: Point
     vss_commitments: List[Point]
 
@@ -235,10 +238,10 @@ def load_local_key(doc: Dict[str, Any], decompress, enc: Encoding = DEFAULT) -> 
     pt = lambda d: enc.point_from(d, decompress)
     return LoadedLocalKey(
         i=int(doc["i"]), t=int(doc["t"]), n=int(doc["n"]), x_i=enc.scalar_from(doc["keys_linear"]["x_i"]),
-        dk=_DK(B(doc["paillier_dk"]["p"]), B(doc["paillier_dk"]["q"])),
+        dk=DecryptionKey(B(doc["paillier_dk"]["p"]), B(doc["paillier_dk"]["q"])),
         pk_vec=[pt(p) for p in doc["pk_vec"]],
-        paillier_key_vec=[_EK(B(e["n"])) for e in doc["paillier_key_vec"]],
-        h1_h2_n_tilde_vec=[_ST(B(s["N"]), B(s["g"]), B(s["ni"])) for s in doc["h1_h2_n_tilde_vec"]],
+        paillier_key_vec=[EncryptionKey(B(e["n"])) for e in doc["paillier_key_vec"]],
+        h1_h2_n_tilde_vec=[DLogStatement(B(s["N"]), B(s["g"]), B(s["ni"])) for s in doc["h1_h2_n_tilde_vec"]],
         y_sum_s=pt(doc["y_sum_s"]), vss_commitments=[pt(p) for p in doc["vss_scheme"]["commitments"]])
 
 
