@@ -428,7 +428,7 @@ int tecdsa_gg18_output_signature_batch(tecdsa_ctx* ctx, int parties, const uint3
  * 2^1022 and p/q < 4), and 2^2046 <= N_tilde < 2^2048, odd.  Any other row makes
  * tecdsa_keys_upload return TECDSA_E_ARG before anything is allocated.                    */
 typedef struct {
-    size_t n_keysets;             /* rows below are indexed by keyset*3 + party (party 0..2)      */
+    size_t n_keysets;             /* rows below are indexed by keyset*3 + party (party 0..2); keyset*parties + party for tecdsa_keys_upload_parties */
     const uint32_t* paillier_p;   /* [rows][32]  DecryptionKey.p  (odd prime, see above)           */
     const uint32_t* paillier_q;   /* [rows][32]  DecryptionKey.q                                   */
     const uint32_t* n_tilde;      /* [rows][64]  DLogStatement.N   (h1_h2_n_tilde_vec)             */
@@ -439,8 +439,16 @@ typedef struct {
     const uint32_t* y;            /* [n_keysets][16]  y_sum_s                                      */
 } tecdsa_keys;
 int tecdsa_keys_upload(tecdsa_ctx* ctx, const tecdsa_keys* keys, tecdsa_keyset** out);
+/* The same for key sets of any size: `parties` (2..64, else TECDSA_E_ARG) rows per key set, row keyset*parties + party, y one row
+ * per key set; validation, derived tables, fixed-base tables and N-adic constants as above.  tecdsa_keys_upload is this call with
+ * parties = 3.  Device memory: every row carries about 48 MB of (h1, h2) fixed-base tables (2 x 368 x 256 x 256 B), so a
+ * 64-party key set takes about 3 GB.  The calls built for three-party key sets (tecdsa_gg20_offline_batch,
+ * tecdsa_gg20_sample_randomness, tecdsa_gg20_offline_records, tecdsa_gg20_sign_batch) refuse any other size with TECDSA_E_ARG;
+ * tecdsa_gg20_offline_general_batch takes every size.                                                                        */
+int tecdsa_keys_upload_parties(tecdsa_ctx* ctx, int parties, const tecdsa_keys* keys, tecdsa_keyset** out);
 int tecdsa_keys_free(tecdsa_ctx* ctx, tecdsa_keyset* ks);
-/* copy one derived per-key table back (test access): 0 = N, 1 = N^2, 5 = p^2, 6 = q^2 ... see csrc/gg20_fields.h */
+/* copy one derived per-key table back (test access, n_keysets * parties rows): 0 = N, 1 = N^2, 5 = p^2, 6 = q^2 ... see
+ * csrc/gg20_fields.h */
 int tecdsa_keys_table(tecdsa_ctx* ctx, const tecdsa_keyset* ks, int table, uint32_t* out_host);
 
 /* Layout (uint32 limb offsets) of one unit's randomness record: every value the reference
@@ -473,6 +481,63 @@ enum {
 int tecdsa_gg20_offline_batch(tecdsa_ctx* ctx, const tecdsa_keyset* ks, const uint32_t* sessions, size_t n_sessions,
                               const uint32_t* rnd, uint8_t* status, uint32_t* R, uint32_t* sigma, uint32_t* t_vec,
                               uint32_t* digest, int mem);
+/* ---- the offline stage for ANY signing set: `OfflineStage` Round0..Round6 (sign/rounds.rs:68-636) for `n_sessions` sessions of
+ * `signers` signers (2 <= signers <= parties of the key set <= 64) of keys in ks, as one call.
+ * sessions = [n_sessions][1 + signers]: the key set, then s_l[p] - 1 (keygen index - 1) of every signer position p.  A key set out
+ * of range, an index >= parties, a repeated index (InvalidSl, sign.rs:87-98), signers < 2 (TooFewParties) or signers > parties
+ * fails the whole call with TECDSA_E_ARG before anything is touched, as does n_sessions * signers > 2^22.
+ * Element u = s*signers + p (E = n_sessions*signers elements).  Inputs, every one drawn as the reference draws it (ranges of
+ * TECDSA_RND_* / tecdsa_gg20_sample_randomness; statement x = keygen party x, N_peer / N~_peer = the peer's key row):
+ *   per element [E][w];  per statement of MessageA's range proofs [parties][E][w] (statement-major);  per pair [signers-1][E][w]
+ *   (peer-major: slab j holds element u towards its j-th peer, position j < p ? j : j + 1).
+ * w_i is not an input: the Lagrange coefficient of every signer, w_i = lambda_i x_i and g_w_vec (SignKeys::create, g_w_vec,
+ * party_i.rs:527-574) are computed on the device from s_l and the key set's x_i / pk rows.
+ * Outputs per element: status (the element's first error, rules of tecdsa_gg20_offline_batch per round: InvalidKey in rounds 1-2,
+ * including MessageB(w)'s key != g_w_vec[j] (rounds.rs:281); TECDSA_ST_PROOF in round 3; TECDSA_ST_COMMITMENT in round 4;
+ * _PDL_VERIFY / _PHASE5_BAD_SUM in round 5; _PHASE6 in round 6), R [16], sigma_i [8] and its own T_i [16]; per session complete
+ * (1 = every member finished).  A session stops in the round in which its first member failed: statuses of later rounds are not
+ * recorded and its R, sigma_i, T_i are zero.
+ * Declared work-saving identities, value-preserving: every receiver runs the same deterministic checks on the same message, so
+ * each element's MessageA range proofs (parties of them) are verified once and serve the 2*(signers-1) MessageB::b that consume
+ * it, each Pedersen proof (round 3), PDL proof (round 5) and HomoElGamal proof (round 6) is verified once; the MessageB
+ * exponentiations for gamma_i and w_i of every pair run as one job list.  Every intermediate lives in stage scratch wiped before
+ * the call returns.  mem = TECDSA_HOST or TECDSA_DEVICE for every buffer of both structs; sessions is read through a host copy. */
+typedef struct {
+    const uint32_t* gamma;            /* [E][8]    gamma_i (SCALAR)                                      */
+    const uint32_t* k;                /* [E][8]    k_i (SCALAR)                                          */
+    const uint32_t* blind;            /* [E][8]    commitment blind (BITS 256)                           */
+    const uint32_t* r_k;              /* [E][64]   Paillier randomness of MessageA (BELOW N_own)         */
+    const uint32_t* l;                /* [E][8]    l_i (SCALAR)                                          */
+    const uint32_t* ped_s1;           /* [E][8]    PedersenProof nonces (SCALAR)                          */
+    const uint32_t* ped_s2;           /* [E][8]                                                          */
+    const uint32_t* heg_s1;           /* [E][8]    HomoELGamalProof nonces (SCALAR)                       */
+    const uint32_t* heg_s2;           /* [E][8]                                                          */
+    const uint32_t* alice_alpha;      /* [parties][E][24]  BELOW q^3                                      */
+    const uint32_t* alice_beta;       /* [parties][E][64]  UNIT(N_own)                                    */
+    const uint32_t* alice_gamma;      /* [parties][E][88]  BELOW q^3 N~_x                                 */
+    const uint32_t* alice_rho;        /* [parties][E][72]  BELOW q N~_x                                   */
+    const uint32_t* beta_tag_gamma;   /* [signers-1][E][64]  BELOW N_peer                                 */
+    const uint32_t* r_gamma;          /* [signers-1][E][64]  BELOW N_peer                                 */
+    const uint32_t* nonce_gamma_b;    /* [signers-1][E][8]   SCALAR                                       */
+    const uint32_t* nonce_gamma_beta; /* [signers-1][E][8]   SCALAR                                       */
+    const uint32_t* beta_tag_w;       /* [signers-1][E][64]                                               */
+    const uint32_t* r_w;              /* [signers-1][E][64]                                               */
+    const uint32_t* nonce_w_b;        /* [signers-1][E][8]                                                */
+    const uint32_t* nonce_w_beta;     /* [signers-1][E][8]                                                */
+    const uint32_t* pdl_alpha;        /* [signers-1][E][24]  BELOW q^3                                    */
+    const uint32_t* pdl_beta;         /* [signers-1][E][64]  RANGE1(N_own)                                */
+    const uint32_t* pdl_rho;          /* [signers-1][E][72]  BELOW q N~_peer                              */
+    const uint32_t* pdl_gamma;        /* [signers-1][E][88]  BELOW q^3 N~_peer                            */
+} tecdsa_offline_general_in;
+typedef struct {
+    uint8_t* status;                  /* [E]                                                             */
+    uint32_t* R;                      /* [E][16]                                                         */
+    uint32_t* sigma;                  /* [E][8]                                                          */
+    uint32_t* T;                      /* [E][16]   the element's own T_i                                 */
+    uint8_t* complete;                /* [n_sessions]                                                    */
+} tecdsa_offline_general_out;
+int tecdsa_gg20_offline_general_batch(tecdsa_ctx* ctx, const tecdsa_keyset* ks, int signers, size_t n_sessions, int mem, const uint32_t* sessions,
+                                      const tecdsa_offline_general_in* in, const tecdsa_offline_general_out* out);
 /* ---- result records, their multi-GPU gather, and the end-to-end call ---------------------------------------------------
  * One 256-byte record per unit (SURVEY.md section 8e) = the fields of CompletedOfflineStage (sign/rounds.rs:647-654) in the
  * reference's byte encodings: status byte, R and t_vec as `Point::to_bytes(true)` (33 bytes), sigma_i and k_i

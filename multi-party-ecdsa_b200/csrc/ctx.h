@@ -60,6 +60,7 @@ struct tecdsa_keyset {
     uint8_t* rec_mem = nullptr;
     const uint8_t* rec[tecdsa::KT_COUNT] = {};
     int n_keysets = 0;
+    int parties = 3;             // key rows per key set: row = keyset * parties + party (tecdsa_keys_upload_parties)
 };
 
 struct tecdsa_ctx {

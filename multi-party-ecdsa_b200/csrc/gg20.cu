@@ -177,12 +177,15 @@ int tecdsa_internal_fb_points_init(int device, cudaStream_t stream, const uint32
 }
 
 // ------------------------------------------------------------------------------------------ keys
-extern "C" int tecdsa_keys_upload(tecdsa_ctx* c, const tecdsa_keys* k, tecdsa_keyset** out) {
+extern "C" int tecdsa_keys_upload(tecdsa_ctx* c, const tecdsa_keys* k, tecdsa_keyset** out) { return tecdsa_keys_upload_parties(c, 3, k, out); }
+extern "C" int tecdsa_keys_upload_parties(tecdsa_ctx* c, int parties, const tecdsa_keys* k, tecdsa_keyset** out) {
     if (!c || !k || !out) return tecdsa_fail(TECDSA_E_ARG, "keys_upload: null argument");
+    if (parties < 2 || parties > 64) return tecdsa_fail(TECDSA_E_ARG, "keys_upload: parties must be in 2..64");
     if (k->n_keysets == 0 || !k->paillier_p || !k->paillier_q || !k->n_tilde || !k->h1 || !k->h2 || !k->x_i || !k->pk || !k->y)
         return tecdsa_fail(TECDSA_E_ARG, "keys_upload: missing table");
     CK(cudaSetDevice(c->device));
-    const int rows = (int)k->n_keysets * 3;
+    if (k->n_keysets > (size_t)(1 << 20)) return tecdsa_fail(TECDSA_E_ARG, "keys_upload: too many key sets");
+    const int rows = (int)k->n_keysets * parties;
     // every modulus must be odd (Montgomery domain), and the key inside the domain of the header: checked on the host copy
     // BEFORE anything is allocated or launched
     for (int r = 0; r < rows; r++) {
@@ -195,6 +198,7 @@ extern "C" int tecdsa_keys_upload(tecdsa_ctx* c, const tecdsa_keys* k, tecdsa_ke
     }
     tecdsa_keyset* ks = new tecdsa_keyset();
     ks->n_keysets = (int)k->n_keysets;
+    ks->parties = parties;
     // from here on every failure releases the partially built key set
 #undef CK
 #define CK(call)                                                                                             \
@@ -284,7 +288,7 @@ extern "C" int tecdsa_keys_free(tecdsa_ctx* c, tecdsa_keyset* ks) {
 }
 extern "C" int tecdsa_keys_table(tecdsa_ctx* c, const tecdsa_keyset* ks, int table, uint32_t* out_host) {
     if (!c || !ks || !out_host || table < 0 || table >= KT_COUNT) return tecdsa_fail(TECDSA_E_ARG, "keys_table: bad argument");
-    CK(cudaMemcpyAsync(out_host, ks->tab[table], (size_t)ks->n_keysets * 3 * KEY_SIZE[table] * 4, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaMemcpyAsync(out_host, ks->tab[table], (size_t)ks->n_keysets * ks->parties * KEY_SIZE[table] * 4, cudaMemcpyDeviceToHost, c->stream));
     CK(cudaStreamSynchronize(c->stream));
     return 0;
 }
@@ -521,6 +525,7 @@ extern "C" int tecdsa_gg20_offline_batch(tecdsa_ctx* c, const tecdsa_keyset* ks,
                                          const uint32_t* rnd, uint8_t* status, uint32_t* R_out, uint32_t* sigma_out,
                                          uint32_t* tvec_out, uint32_t* digest_out, int mem) {
     if (!c || !ks || !sessions || !rnd || !status) return tecdsa_fail(TECDSA_E_ARG, "gg20_offline: null argument");
+    if (ks->parties != 3) return tecdsa_fail(TECDSA_E_ARG, "gg20_offline: the key set must have three parties");
     if (mem != TECDSA_HOST && mem != TECDSA_DEVICE) return tecdsa_fail(TECDSA_E_ARG, "gg20_offline: bad mem");
     if (n_sessions == 0) return 0;
     if (n_sessions > (1u << 22)) return tecdsa_fail(TECDSA_E_ARG, "gg20_offline: too many sessions");

@@ -4,6 +4,7 @@
 // driver uses (jobs.cuh, modinv.cuh, gg20_glue.cuh); results are canonical residues /
 // proof bytes identical to the L3 path and to the oracle.
 #include "stage.cuh"
+#include "l12_steps.h"
 
 using namespace tecdsa;
 
@@ -358,9 +359,14 @@ extern "C" int tecdsa_secp_mul_batch(tecdsa_ctx* c, const uint32_t* points, cons
     const uint32_t *dp = S.in(points, count * 16), *dk = S.in(scalars, count * 8);
     uint32_t* dout = S.out(out, count * 16);
     if (S.err) return S.err;
-    k_secp_mul<<<grid_for(count), 64, 0, c->stream>>>(dout, dp, dk, (int)count);
-    KCHECK();
+    RUN(secp_mul_step(c, (int)count, dp, dk, dout));
     return S.finish();
+}
+// out = k P (k G for pts == NULL) on device-resident arrays
+int tecdsa::secp_mul_step(tecdsa_ctx* c, int n, const uint32_t* pts, const uint32_t* scalars, uint32_t* out) {
+    k_secp_mul<<<grid_for((size_t)n), 64, 0, c->stream>>>(out, pts, scalars, n);
+    KCHECK();
+    return 0;
 }
 
 // ------------------------------------------------------------------------------------------ L1: Paillier
@@ -429,8 +435,8 @@ extern "C" int tecdsa_paillier_decrypt_batch(tecdsa_ctx* c, const tecdsa_keyset*
 }
 
 // ------------------------------------------------------------------------------------------ L2: MtA range proof (Alice)
-// AliceProof::generate on device-resident arrays (shared by the L2 entry point and tecdsa_mta_message_a_batch)
-static int alice_generate_dev(tecdsa_ctx* c, Stage& S, const tecdsa_keyset* ks, int n, const uint32_t* er, const uint32_t* sr, const uint32_t* da,
+// AliceProof::generate on device-resident arrays (shared by the L2 entry point, tecdsa_mta_message_a_batch and the general offline stage)
+int tecdsa::alice_generate_step(tecdsa_ctx* c, Stage& S, const tecdsa_keyset* ks, int n, const uint32_t* er, const uint32_t* sr, const uint32_t* da,
                               const uint32_t* dc, const uint32_t* dr, const uint32_t* dal, const uint32_t* dbe, const uint32_t* dga, const uint32_t* dro,
                               uint32_t* dz, uint32_t* de, uint32_t* ds, uint32_t* ds1, uint32_t* ds2) {
     const size_t count = (size_t)n;
@@ -465,12 +471,12 @@ extern "C" int tecdsa_alice_proof_generate_batch(tecdsa_ctx* c, const tecdsa_key
                    *dro = S.in(rho, count * 72);
     uint32_t *dz = S.out(z, count * 64), *de = S.out(e, count * 8), *ds = S.out(s, count * 64), *ds1 = S.out(s1, count * 28), *ds2 = S.out(s2, count * 92);
     if (S.err) return S.err;
-    RUN(alice_generate_dev(c, S, ks, (int)count, er, sr, da, dc, dr, dal, dbe, dga, dro, dz, de, ds, ds1, ds2));
+    RUN(alice_generate_step(c, S, ks, (int)count, er, sr, da, dc, dr, dal, dbe, dga, dro, dz, de, ds, ds1, ds2));
     return S.finish();
 }
 
-// AliceProof::verify on device-resident arrays (shared by the L2 entry point and tecdsa_mta_message_b_batch)
-static int alice_verify_dev(tecdsa_ctx* c, Stage& S, const tecdsa_keyset* ks, int n, const uint32_t* er, const uint32_t* sr, const uint32_t* dc,
+// AliceProof::verify on device-resident arrays (shared by the L2 entry point, tecdsa_mta_message_b_batch and the general offline stage)
+int tecdsa::alice_verify_step(tecdsa_ctx* c, Stage& S, const tecdsa_keyset* ks, int n, const uint32_t* er, const uint32_t* sr, const uint32_t* dc,
                             const uint32_t* dz, const uint32_t* de, const uint32_t* ds, const uint32_t* ds1, const uint32_t* ds2, uint8_t* dst) {
     const size_t count = (size_t)n;
     uint32_t *gs1 = S.tmp<uint32_t>(count * 128), *ze = S.tmp<uint32_t>(count * 64), *ce = S.tmp<uint32_t>(count * 128),
@@ -511,7 +517,7 @@ extern "C" int tecdsa_alice_proof_verify_batch(tecdsa_ctx* c, const tecdsa_keyse
                    *de = S.in(e, count * 8), *ds = S.in(s, count * 64), *ds1 = S.in(s1, count * 28), *ds2 = S.in(s2, count * 92);
     uint8_t* dst = S.out(status, count);
     if (S.err) return S.err;
-    RUN(alice_verify_dev(c, S, ks, (int)count, er, sr, dc, dz, de, ds, ds1, ds2, dst));
+    RUN(alice_verify_step(c, S, ks, (int)count, er, sr, dc, dz, de, ds, ds1, ds2, dst));
     return S.finish();
 }
 
@@ -529,6 +535,16 @@ extern "C" int tecdsa_pdl_prove_batch(tecdsa_ctx* c, const tecdsa_keyset* ks, co
                    *dro = S.in(rho, count * 72), *dga = S.in(gamma, count * 88);
     uint32_t *dz = S.out(z, count * 64), *du1 = S.out(u1, count * 16), *du2 = S.out(u2, count * 128), *du3 = S.out(u3, count * 64),
              *ds1 = S.out(s1, count * 28), *ds2 = S.out(s2, count * 64), *ds3 = S.out(s3, count * 92);
+    if (S.err) return S.err;
+    RUN(pdl_prove_step(c, S, ks, n, er, sr, dx, dr, dc, dQ, dG, dal, dbe, dro, dga, dz, du1, du2, du3, ds1, ds2, ds3));
+    return S.finish();
+}
+
+// PDLwSlackProof::prove on device-resident arrays
+int tecdsa::pdl_prove_step(tecdsa_ctx* c, Stage& S, const tecdsa_keyset* ks, int n, const uint32_t* er, const uint32_t* sr, const uint32_t* dx, const uint32_t* dr,
+                   const uint32_t* dc, const uint32_t* dQ, const uint32_t* dG, const uint32_t* dal, const uint32_t* dbe, const uint32_t* dro,
+                   const uint32_t* dga, uint32_t* dz, uint32_t* du1, uint32_t* du2, uint32_t* du3, uint32_t* ds1, uint32_t* ds2, uint32_t* ds3) {
+    const size_t count = (size_t)n;
     uint32_t *lin = S.tmp<uint32_t>(count * 128), *e = S.tmp<uint32_t>(count * 8);
     if (S.err) return S.err;
     Arena A = key_arena(ks);
@@ -543,7 +559,7 @@ extern "C" int tecdsa_pdl_prove_batch(tecdsa_ctx* c, const tecdsa_keyset* ks, co
     KCHECK();
     add_exp(L.e64, 64, n, tab(ks->tab[KT_N], er, 64), 1, arr(dr, 64), arr(e, 8), 8, NONE, NONE, 0, 1, arr(dbe, 64), NONE, ds2, 64);   // s2 = r^e beta mod N (:113)
     RUN(run(c, L.e64, 64));
-    return S.finish();
+    return 0;
 }
 
 extern "C" int tecdsa_pdl_verify_batch(tecdsa_ctx* c, const tecdsa_keyset* ks, const uint32_t* ek_row, const uint32_t* st_row, const uint32_t* cipher,
@@ -557,6 +573,16 @@ extern "C" int tecdsa_pdl_verify_batch(tecdsa_ctx* c, const tecdsa_keyset* ks, c
                    *dz = S.in(z, count * 64), *du1 = S.in(u1, count * 16), *du2 = S.in(u2, count * 128), *du3 = S.in(u3, count * 64),
                    *ds1 = S.in(s1, count * 28), *ds2 = S.in(s2, count * 64), *ds3 = S.in(s3, count * 92);
     uint8_t* dst = S.out(status, count);
+    if (S.err) return S.err;
+    RUN(pdl_verify_step(c, S, ks, n, er, sr, dc, dQ, dG, dz, du1, du2, du3, ds1, ds2, ds3, dst));
+    return S.finish();
+}
+
+// PDLwSlackProof::verify on device-resident arrays
+int tecdsa::pdl_verify_step(tecdsa_ctx* c, Stage& S, const tecdsa_keyset* ks, int n, const uint32_t* er, const uint32_t* sr, const uint32_t* dc, const uint32_t* dQ,
+                    const uint32_t* dG, const uint32_t* dz, const uint32_t* du1, const uint32_t* du2, const uint32_t* du3, const uint32_t* ds1,
+                    const uint32_t* ds2, const uint32_t* ds3, uint8_t* dst) {
+    const size_t count = (size_t)n;
     uint32_t *e = S.tmp<uint32_t>(count * 8), *lin = S.tmp<uint32_t>(count * 128), *ze = S.tmp<uint32_t>(count * 64), *ce = S.tmp<uint32_t>(count * 128),
              *zei = S.tmp<uint32_t>(count * 64), *cei = S.tmp<uint32_t>(count * 128), *u2t = S.tmp<uint32_t>(count * 128), *u3t = S.tmp<uint32_t>(count * 64);
     uint8_t *okz = S.tmp<uint8_t>(count), *okc = S.tmp<uint8_t>(count);
@@ -577,7 +603,7 @@ extern "C" int tecdsa_pdl_verify_batch(tecdsa_ctx* c, const tecdsa_keyset* ks, c
     RUN(run_nn(c, L.e128)); RUN(run(c, L.e64, 64));
     k_pdl_vpost<<<grid_for(count), 64, 0, c->stream>>>(dG, dQ, du1, du2, du3, ds1, e, u2t, u3t, okz, okc, dst, n);
     KCHECK();
-    return S.finish();
+    return 0;
 }
 
 // ------------------------------------------------------------------------------------------ L2: Bob's range proof (MtA / MtAwc)
@@ -689,9 +715,13 @@ extern "C" int tecdsa_pedersen_prove_batch(tecdsa_ctx* c, const uint32_t* m, con
     const uint32_t *dm = S.in(m, count * 8), *dr = S.in(r, count * 8), *d1 = S.in(s1, count * 8), *d2 = S.in(s2, count * 8);
     uint32_t *dc = S.out(com, count * 16), *dp = S.out(proof, count * 64);
     if (S.err) return S.err;
-    k_pedersen_prove<<<grid_for(count), 64, 0, c->stream>>>(dc, dp, dm, dr, d1, d2, (int)count);
-    KCHECK();
+    RUN(pedersen_prove_step(c, (int)count, dm, dr, d1, d2, dc, dp));
     return S.finish();
+}
+int tecdsa::pedersen_prove_step(tecdsa_ctx* c, int n, const uint32_t* m, const uint32_t* r, const uint32_t* s1, const uint32_t* s2, uint32_t* com, uint32_t* proof) {
+    k_pedersen_prove<<<grid_for((size_t)n), 64, 0, c->stream>>>(com, proof, m, r, s1, s2, n);
+    KCHECK();
+    return 0;
 }
 extern "C" int tecdsa_pedersen_verify_batch(tecdsa_ctx* c, const uint32_t* com, const uint32_t* proof, uint8_t* status, size_t count, int mem) {
     if (!com || !proof || !status) return tecdsa_fail(TECDSA_E_ARG, "pedersen_verify: null argument");
@@ -699,9 +729,13 @@ extern "C" int tecdsa_pedersen_verify_batch(tecdsa_ctx* c, const uint32_t* com, 
     const uint32_t *dc = S.in(com, count * 16), *dp = S.in(proof, count * 64);
     uint8_t* o = S.out(status, count);
     if (S.err) return S.err;
-    k_pedersen_verify<<<grid_for(count), 64, 0, c->stream>>>(dc, dp, o, (int)count);
-    KCHECK();
+    RUN(pedersen_verify_step(c, (int)count, dc, dp, o));
     return S.finish();
+}
+int tecdsa::pedersen_verify_step(tecdsa_ctx* c, int n, const uint32_t* com, const uint32_t* proof, uint8_t* status) {
+    k_pedersen_verify<<<grid_for((size_t)n), 64, 0, c->stream>>>(com, proof, status, n);
+    KCHECK();
+    return 0;
 }
 extern "C" int tecdsa_heg_prove_batch(tecdsa_ctx* c, const uint32_t* G, const uint32_t* D, const uint32_t* E, const uint32_t* x, const uint32_t* r,
                                       const uint32_t* s1, const uint32_t* s2, uint32_t* proof, size_t count, int mem) {
@@ -711,9 +745,14 @@ extern "C" int tecdsa_heg_prove_batch(tecdsa_ctx* c, const uint32_t* G, const ui
                    *d1 = S.in(s1, count * 8), *d2 = S.in(s2, count * 8);
     uint32_t* o = S.out(proof, count * 48);
     if (S.err) return S.err;
-    k_heg_prove<<<grid_for(count), 64, 0, c->stream>>>(o, dG, dD, dE, dx, dr, d1, d2, (int)count);
-    KCHECK();
+    RUN(heg_prove_step(c, (int)count, dG, dD, dE, dx, dr, d1, d2, o));
     return S.finish();
+}
+int tecdsa::heg_prove_step(tecdsa_ctx* c, int n, const uint32_t* G, const uint32_t* D, const uint32_t* E, const uint32_t* x, const uint32_t* r, const uint32_t* s1,
+                   const uint32_t* s2, uint32_t* proof) {
+    k_heg_prove<<<grid_for((size_t)n), 64, 0, c->stream>>>(proof, G, D, E, x, r, s1, s2, n);
+    KCHECK();
+    return 0;
 }
 extern "C" int tecdsa_heg_verify_batch(tecdsa_ctx* c, const uint32_t* G, const uint32_t* D, const uint32_t* E, const uint32_t* proof, uint8_t* status,
                                        size_t count, int mem) {
@@ -722,9 +761,13 @@ extern "C" int tecdsa_heg_verify_batch(tecdsa_ctx* c, const uint32_t* G, const u
     const uint32_t *dG = S.in(G, count * 16), *dD = S.in(D, count * 16), *dE = S.in(E, count * 16), *dp = S.in(proof, count * 48);
     uint8_t* o = S.out(status, count);
     if (S.err) return S.err;
-    k_heg_verify<<<grid_for(count), 64, 0, c->stream>>>(dp, dG, dD, dE, o, (int)count);
-    KCHECK();
+    RUN(heg_verify_step(c, (int)count, dG, dD, dE, dp, o));
     return S.finish();
+}
+int tecdsa::heg_verify_step(tecdsa_ctx* c, int n, const uint32_t* G, const uint32_t* D, const uint32_t* E, const uint32_t* proof, uint8_t* status) {
+    k_heg_verify<<<grid_for((size_t)n), 64, 0, c->stream>>>(proof, G, D, E, status, n);
+    KCHECK();
+    return 0;
 }
 extern "C" int tecdsa_sha256_bigints_batch(tecdsa_ctx* c, const uint32_t* data, const int* item_limbs, int n_items, uint32_t* digest, size_t count, int mem) {
     if (!data || !item_limbs || !digest || n_items <= 0 || n_items > 64) return tecdsa_fail(TECDSA_E_ARG, "sha256_bigints: bad argument");
@@ -746,9 +789,13 @@ extern "C" int tecdsa_hash_commitment_batch(tecdsa_ctx* c, const uint32_t* point
     const uint32_t *dp = S.in(points, count * 16), *db = S.in(blind, count * 8);
     uint32_t* o = S.out(com, count * 8);
     if (S.err) return S.err;
-    k_hash_commit<<<grid_for(count), 64, 0, c->stream>>>(dp, db, o, (int)count);
-    KCHECK();
+    RUN(hash_commitment_step(c, (int)count, dp, db, o));
     return S.finish();
+}
+int tecdsa::hash_commitment_step(tecdsa_ctx* c, int n, const uint32_t* points, const uint32_t* blind, uint32_t* com) {
+    k_hash_commit<<<grid_for((size_t)n), 64, 0, c->stream>>>(points, blind, com, n);
+    KCHECK();
+    return 0;
 }
 
 
@@ -760,13 +807,21 @@ extern "C" int tecdsa_mta_message_a_batch(tecdsa_ctx* c, const tecdsa_keyset* ks
     if (!c || !ks || !ek_row || !a || !r || !c_out || n_st < 0 || n_st > 16) return tecdsa_fail(TECDSA_E_ARG, "mta_message_a: bad argument");
     if (n_st > 0 && (!st_rows || !alpha || !beta || !gamma || !rho || !z || !e || !s || !s1 || !s2)) return tecdsa_fail(TECDSA_E_ARG, "mta_message_a: null proof buffer");
     STAGE_PROLOGUE("mta_message_a", count);
-    const int n = (int)count;
     const size_t np = count * (size_t)n_st;
     const uint32_t *er = S.in(ek_row, count), *da = S.in(a, count * 8), *dr = S.in(r, count * 64);
     uint32_t* dc = S.out(c_out, count * 128);
+    const uint32_t *sr = S.in(st_rows, np), *dal = S.in(alpha, np * 24), *dbe = S.in(beta, np * 64), *dga = S.in(gamma, np * 88), *dro = S.in(rho, np * 72);
+    uint32_t *dz = S.out(z, np * 64), *de = S.out(e, np * 8), *ds = S.out(s, np * 64), *ds1 = S.out(s1, np * 28), *ds2 = S.out(s2, np * 92);
+    if (S.err) return S.err;
+    RUN(mta_message_a_step(c, S, ks, (int)count, n_st, er, da, dr, sr, dal, dbe, dga, dro, dc, dz, de, ds, ds1, ds2));
+    return S.finish();
+}
+
+// c = Enc(a; r) = (1 + a N) r^N mod N^2 under key rows er (mod.rs:68-75), on device-resident arrays
+int tecdsa::mta_encrypt_step(tecdsa_ctx* c, Stage& S, const tecdsa_keyset* ks, int n, const uint32_t* er, const uint32_t* da, const uint32_t* dr, uint32_t* dc) {
+    const size_t count = (size_t)n;
     uint32_t *a64 = S.tmp<uint32_t>(count * 64), *lin = S.tmp<uint32_t>(count * 128);
     if (S.err) return S.err;
-    // c = (1 + a N) r^N mod N^2   (mod.rs:68-75)
     CK(cudaMemsetAsync(a64, 0, count * 64 * 4, c->stream));
     CK(cudaMemcpy2DAsync(a64, 64 * 4, da, 8 * 4, 8 * 4, count, cudaMemcpyDeviceToDevice, c->stream));
     k_lin<<<grid_for(count), 64, 0, c->stream>>>(lin, a64, 64, ks->tab[KT_N], er, n);
@@ -774,9 +829,16 @@ extern "C" int tecdsa_mta_message_a_batch(tecdsa_ctx* c, const tecdsa_keyset* ks
     Launches L;
     add_nn(L.e128, n, key_n(ks, er), key_nadic(ks, er), 1, arr(dr, 64), tab(ks->tab[KT_N], er, 64), 64, NONE, NONE, 0, 1, arr(lin, 128), NONE, dc, 128);
     RUN(run_nn(c, L.e128));
+    return 0;
+}
+
+// MessageA::a (mod.rs:52-80) on device-resident arrays: c, and one AliceProof per (instance, statement), instance-major
+int tecdsa::mta_message_a_step(tecdsa_ctx* c, Stage& S, const tecdsa_keyset* ks, int n, int n_st, const uint32_t* er, const uint32_t* da, const uint32_t* dr,
+                       const uint32_t* sr, const uint32_t* dal, const uint32_t* dbe, const uint32_t* dga, const uint32_t* dro, uint32_t* dc, uint32_t* dz,
+                       uint32_t* de, uint32_t* ds, uint32_t* ds1, uint32_t* ds2) {
+    const size_t count = (size_t)n, np = count * (size_t)n_st;
+    RUN(mta_encrypt_step(c, S, ks, n, er, da, dr, dc));
     if (n_st > 0) {
-        const uint32_t *sr = S.in(st_rows, np), *dal = S.in(alpha, np * 24), *dbe = S.in(beta, np * 64), *dga = S.in(gamma, np * 88), *dro = S.in(rho, np * 72);
-        uint32_t *dz = S.out(z, np * 64), *de = S.out(e, np * 8), *ds = S.out(s, np * 64), *ds1 = S.out(s1, np * 28), *ds2 = S.out(s2, np * 92);
         uint32_t *er_f = S.tmp<uint32_t>(np), *a_f = S.tmp<uint32_t>(np * 8), *r_f = S.tmp<uint32_t>(np * 64), *c_f = S.tmp<uint32_t>(np * 128);
         if (S.err) return S.err;
         const int g = grid_for(np);
@@ -785,9 +847,9 @@ extern "C" int tecdsa_mta_message_a_batch(tecdsa_ctx* c, const tecdsa_keyset* ks
         k_expand<<<g, 64, 0, c->stream>>>(r_f, dr, 64, n_st, n);
         k_expand<<<g, 64, 0, c->stream>>>(c_f, dc, 128, n_st, n);
         KCHECK();
-        RUN(alice_generate_dev(c, S, ks, (int)np, er_f, sr, a_f, c_f, r_f, dal, dbe, dga, dro, dz, de, ds, ds1, ds2));
+        RUN(alice_generate_step(c, S, ks, (int)np, er_f, sr, a_f, c_f, r_f, dal, dbe, dga, dro, dz, de, ds, ds1, ds2));
     }
-    return S.finish();
+    return 0;
 }
 
 extern "C" int tecdsa_mta_message_b_batch(tecdsa_ctx* c, const tecdsa_keyset* ks, const uint32_t* ek_row, const uint32_t* st_rows, int n_st,
@@ -800,23 +862,35 @@ extern "C" int tecdsa_mta_message_b_batch(tecdsa_ctx* c, const tecdsa_keyset* ks
         return tecdsa_fail(TECDSA_E_ARG, "mta_message_b: bad argument");
     if (n_st > 0 && (!st_rows || !z || !e || !s || !s1 || !s2)) return tecdsa_fail(TECDSA_E_ARG, "mta_message_b: null proof buffer");
     STAGE_PROLOGUE("mta_message_b", count);
-    const int n = (int)count;
     const size_t np = count * (size_t)n_st;
     const uint32_t *er = S.in(ek_row, count), *db = S.in(b, count * 8), *dca = S.in(c_a, count * 128), *dr = S.in(randomness, count * 64),
                    *dbt = S.in(beta_tag, count * 64), *dnb = S.in(nonce_b, count * 8), *dnt = S.in(nonce_beta, count * 8);
+    const uint32_t *sr = S.in(st_rows, np), *dz = S.in(z, np * 64), *de = S.in(e, np * 8), *ds = S.in(s, np * 64), *ds1 = S.in(s1, np * 28), *ds2 = S.in(s2, np * 92);
     uint32_t *dcb = S.out(c_b, count * 128), *dbp = S.out(b_proof, count * 40), *dtp = S.out(beta_tag_proof, count * 40), *dbeta = S.out(beta, count * 8);
     uint8_t* dst = S.out(status, count);
-    uint8_t* pst = S.tmp<uint8_t>(np ? np : 1);
+    if (S.err) return S.err;
+    RUN(mta_message_b_step(c, S, ks, (int)count, er, db, dca, dr, dbt, dnb, dnt, n_st, sr, dz, de, ds, ds1, ds2, nullptr, dcb, dbp, dtp, dbeta, dst));
+    return S.finish();
+}
+
+// MessageB::b (mod.rs:84-148) on device-resident arrays.  The n_st range proofs of instance i's MessageA are verified here
+// (instance-major, as tecdsa_mta_message_b_batch takes them), unless `checked` already holds their statuses ([n][n_st]): a caller
+// that answers one MessageA several times verifies its proofs once.
+int tecdsa::mta_message_b_step(tecdsa_ctx* c, Stage& S, const tecdsa_keyset* ks, int n, const uint32_t* er, const uint32_t* db, const uint32_t* dca, const uint32_t* dr,
+                       const uint32_t* dbt, const uint32_t* dnb, const uint32_t* dnt, int n_st, const uint32_t* sr, const uint32_t* dz, const uint32_t* de,
+                       const uint32_t* ds, const uint32_t* ds1, const uint32_t* ds2, const uint8_t* checked, uint32_t* dcb, uint32_t* dbp, uint32_t* dtp,
+                       uint32_t* dbeta, uint8_t* dst) {
+    const size_t count = (size_t)n, np = count * (size_t)n_st;
+    uint8_t* pst = checked ? nullptr : S.tmp<uint8_t>(np ? np : 1);
     uint32_t* lin = S.tmp<uint32_t>(count * 128);
     if (S.err) return S.err;
-    if (n_st > 0) {     // verify every range proof of MessageA (mod.rs:123-131)
-        const uint32_t *sr = S.in(st_rows, np), *dz = S.in(z, np * 64), *de = S.in(e, np * 8), *ds = S.in(s, np * 64), *ds1 = S.in(s1, np * 28), *ds2 = S.in(s2, np * 92);
+    if (n_st > 0 && !checked) {     // verify every range proof of MessageA (mod.rs:123-131)
         uint32_t *er_f = S.tmp<uint32_t>(np), *c_f = S.tmp<uint32_t>(np * 128);
         if (S.err) return S.err;
         k_expand<<<grid_for(np), 64, 0, c->stream>>>(er_f, er, 1, n_st, n);
         k_expand<<<grid_for(np), 64, 0, c->stream>>>(c_f, dca, 128, n_st, n);
         KCHECK();
-        RUN(alice_verify_dev(c, S, ks, (int)np, er_f, sr, c_f, dz, de, ds, ds1, ds2, pst));
+        RUN(alice_verify_step(c, S, ks, (int)np, er_f, sr, c_f, dz, de, ds, ds1, ds2, pst));
     }
     // c_b = c_a^b * Enc(beta'; r') mod N^2   (mod.rs:133-145)
     k_lin<<<grid_for(count), 64, 0, c->stream>>>(lin, dbt, 64, ks->tab[KT_N], er, n);
@@ -824,9 +898,9 @@ extern "C" int tecdsa_mta_message_b_batch(tecdsa_ctx* c, const tecdsa_keyset* ks
     Launches L;
     add_nn(L.e128, n, key_n(ks, er), key_nadic(ks, er), 2, arr(dr, 64), tab(ks->tab[KT_N], er, 64), 64, arr(dca, 128), arr(db, 8), 8, 1, arr(lin, 128), NONE, dcb, 128);
     RUN(run_nn(c, L.e128));
-    k_mta_b_post<<<grid_for(count), 64, 0, c->stream>>>(pst, n_st, db, dbt, dnb, dnt, dbeta, dbp, dtp, dst, n);
+    k_mta_b_post<<<grid_for(count), 64, 0, c->stream>>>(checked ? checked : pst, n_st, db, dbt, dnb, dnt, dbeta, dbp, dtp, dst, n);
     KCHECK();
-    return S.finish();
+    return 0;
 }
 
 extern "C" int tecdsa_mta_get_alpha_batch(tecdsa_ctx* c, const tecdsa_keyset* ks, const uint32_t* dk_row, const uint32_t* a, const uint32_t* c_b,
@@ -834,11 +908,19 @@ extern "C" int tecdsa_mta_get_alpha_batch(tecdsa_ctx* c, const tecdsa_keyset* ks
                                           uint8_t* status, size_t count, int mem) {
     if (!c || !ks || !dk_row || !a || !c_b || !b_proof || !beta_tag_proof || !alpha || !status) return tecdsa_fail(TECDSA_E_ARG, "mta_get_alpha: null argument");
     STAGE_PROLOGUE("mta_get_alpha", count);
-    const int n = (int)count;
     const uint32_t *dr = S.in(dk_row, count), *da = S.in(a, count * 8), *dcb = S.in(c_b, count * 128), *dbp = S.in(b_proof, count * 40), *dtp = S.in(beta_tag_proof, count * 40);
     uint32_t* dal = S.out(alpha, count * 8);
     uint32_t* dpl = alpha_plain ? S.out(alpha_plain, count * 64) : S.tmp<uint32_t>(count * 64);
     uint8_t* dst = S.out(status, count);
+    if (S.err) return S.err;
+    RUN(mta_get_alpha_step(c, S, ks, (int)count, dr, da, dcb, dbp, dtp, dal, dpl, dst));
+    return S.finish();
+}
+
+// MessageB::verify_proofs_get_alpha (mod.rs:150-179) on device-resident arrays
+int tecdsa::mta_get_alpha_step(tecdsa_ctx* c, Stage& S, const tecdsa_keyset* ks, int n, const uint32_t* dr, const uint32_t* da, const uint32_t* dcb, const uint32_t* dbp,
+                       const uint32_t* dtp, uint32_t* dal, uint32_t* dpl, uint8_t* dst) {
+    const size_t count = (size_t)n;
     uint32_t *dp = S.tmp<uint32_t>(count * 64), *dq = S.tmp<uint32_t>(count * 64);
     if (S.err) return S.err;
     Launches L;
@@ -846,6 +928,5 @@ extern "C" int tecdsa_mta_get_alpha_batch(tecdsa_ctx* c, const tecdsa_keyset* ks
     RUN(run_nn(c, L.e128, 32));
     k_mta_alpha<<<grid_for(count), 64, 0, c->stream>>>(key_arena(ks), dr, dp, dq, da, dbp, dtp, dpl, dal, dst, n);
     KCHECK();
-    return S.finish();
+    return 0;
 }
-

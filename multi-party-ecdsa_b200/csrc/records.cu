@@ -194,6 +194,7 @@ extern "C" int tecdsa_gather_results(tecdsa_ctx* c, void* nccl_comm, const uint8
 extern "C" int tecdsa_gg20_offline_records(tecdsa_ctx* c, const tecdsa_keyset* ks, void* nccl_comm, const uint32_t* sessions, size_t n_sessions,
                                            const uint32_t* rnd, uint8_t* all_records, int mem) {
     if (!c || !ks || !sessions || !rnd || !all_records) return tecdsa_fail(TECDSA_E_ARG, "gg20_offline_records: null argument");
+    if (ks->parties != 3) return tecdsa_fail(TECDSA_E_ARG, "gg20_offline_records: the key set must have three parties");
     if (mem != TECDSA_HOST && mem != TECDSA_DEVICE) return tecdsa_fail(TECDSA_E_ARG, "gg20_offline_records: bad mem");
     if (n_sessions == 0) return 0;
     if (n_sessions > (1u << 22)) return tecdsa_fail(TECDSA_E_ARG, "gg20_offline_records: too many sessions");
@@ -247,6 +248,7 @@ extern "C" int tecdsa_gg20_sign_batch(tecdsa_ctx* c, const tecdsa_keyset* ks, co
                                       const uint32_t* R, const uint32_t* sigma, const uint32_t* k, uint32_t* s_i, uint32_t* sig_r, uint32_t* sig_s,
                                       uint8_t* recid, uint8_t* status, int mem) {
     if (!c || !ks || !sessions || !message || !R || !sigma || !k || !sig_r || !sig_s || !recid || !status) return tecdsa_fail(TECDSA_E_ARG, "gg20_sign: null argument");
+    if (ks->parties != 3) return tecdsa_fail(TECDSA_E_ARG, "gg20_sign: the key set must have three parties");
     STAGE_PROLOGUE("gg20_sign", n_sessions);
     const size_t U = 2 * n_sessions;
     const uint32_t *dsess = S.in(sessions, n_sessions * 3), *dm = S.in(message, n_sessions * 8), *dR = S.in(R, U * 16), *dsg = S.in(sigma, U * 8), *dk = S.in(k, U * 8);

@@ -82,6 +82,7 @@ extern "C" int tecdsa_sample_batch(tecdsa_ctx* c, const uint32_t seed[8], uint64
 extern "C" int tecdsa_gg20_sample_randomness(tecdsa_ctx* c, const tecdsa_keyset* ks, const uint32_t* sessions, size_t n_sessions, const uint32_t seed[8],
                                              uint64_t first_unit, uint32_t* rnd, uint8_t* status, int mem) {
     if (!ks || !sessions || !seed || !rnd || !status) return tecdsa_fail(TECDSA_E_ARG, "gg20_sample_randomness: null argument");
+    if (ks->parties != 3) return tecdsa_fail(TECDSA_E_ARG, "gg20_sample_randomness: the key set must have three parties");
     if (n_sessions > (1u << 22)) return tecdsa_fail(TECDSA_E_ARG, "gg20_sample_randomness: too many sessions");
     STAGE_PROLOGUE("gg20_sample_randomness", n_sessions);
     const size_t U = 2 * n_sessions;

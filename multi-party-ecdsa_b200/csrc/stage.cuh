@@ -9,11 +9,11 @@
 #include <vector>
 
 using namespace tecdsa;      // internal header, included by .cu files only
-namespace {
+namespace tecdsa {
 
-// Stream-ordered staging of caller buffers: HOST pointers are copied to device scratch (and
-// results copied back by finish()), DEVICE pointers are used in place.  finish() runs once: an
-// entry point calls it on its success return, and the destructor runs it on every other exit.
+// Stream-ordered staging of caller buffers (in a named namespace: the step functions of l12_steps.h take it across units).
+// HOST pointers are copied to device scratch (and results copied back by finish()), DEVICE pointers are used in place.
+// finish() runs once: an entry point calls it on its success return, and the destructor runs it on every other exit.
 struct Stage {
     tecdsa_ctx* c;
     int mem;
@@ -63,6 +63,9 @@ struct Stage {
         return err;
     }
 };
+
+}  // namespace tecdsa
+namespace {
 
 const Operand NONE = {nullptr, nullptr, 0, 0, 0};
 Operand arr(const uint32_t* p, uint32_t limbs) { return Operand{p, nullptr, limbs, 0, limbs}; }

@@ -35,6 +35,7 @@ def _bind(lib):
     if getattr(lib, "_gg20_bound", False):
         return
     lib.tecdsa_keys_upload.argtypes = [ctypes.c_void_p, ctypes.POINTER(_Keys), ctypes.POINTER(ctypes.c_void_p)]
+    lib.tecdsa_keys_upload_parties.argtypes = [ctypes.c_void_p, ctypes.c_int, ctypes.POINTER(_Keys), ctypes.POINTER(ctypes.c_void_p)]
     lib.tecdsa_keys_free.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
     lib.tecdsa_keys_table.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]
     lib.tecdsa_gg20_offline_batch.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t] + [ctypes.c_void_p] * 6 + [ctypes.c_int]
@@ -52,12 +53,20 @@ def unpack_point(v: int):
 
 
 class KeySets:
-    """Device-resident LocalKey material of several (t=1,n=3) key sets.  `keysets[k]` is a list of
-    three objects with the fields of the reference's LocalKey (i, x_i, dk.p, dk.q, pk_vec,
-    h1_h2_n_tilde_vec, y_sum_s) — e.g. oracle.LocalKey or any duck-typed equivalent."""
+    """Device-resident LocalKey material of several key sets of one size n (2..64 parties; key row = keyset * n + party).
+    `keysets[k]` is a list of n objects with the fields of the reference's LocalKey (i, x_i, dk.p, dk.q, pk_vec,
+    h1_h2_n_tilde_vec, y_sum_s) — e.g. oracle.LocalKey or any duck-typed equivalent.  Three-party key sets go through
+    tecdsa_keys_upload (what the t = 1, two-signer calls take), other sizes through tecdsa_keys_upload_parties.  Every key row
+    carries about 48 MB of device tables."""
 
     def __init__(self, eng: Engine, keysets: Sequence[Sequence]):
         _bind(eng.lib)
+        sizes = {len(ks) for ks in keysets}
+        if len(sizes) > 1:
+            raise ValueError(f"KeySets: key sets of one size only, got sizes {sorted(sizes)}")
+        self.parties = sizes.pop() if sizes else 3
+        if not 2 <= self.parties <= 64:
+            raise ValueError(f"KeySets: a key set has 2..64 parties, got {self.parties}")
         self.eng = eng
         self.n = len(keysets)
         rows = [lk for ks in keysets for lk in ks]
@@ -71,10 +80,13 @@ class KeySets:
             y=ints_to_limbs([pack_point(ks[0].y_sum_s) for ks in keysets], 16))
         k = _Keys(self.n, *[self._bufs[n].ctypes.data for n in ("paillier_p", "paillier_q", "n_tilde", "h1", "h2", "x_i", "pk", "y")])
         self.handle = ctypes.c_void_p()
-        eng._ck(eng.lib.tecdsa_keys_upload(eng._ctx, ctypes.byref(k), ctypes.byref(self.handle)), "keys_upload")
+        if self.parties == 3:
+            eng._ck(eng.lib.tecdsa_keys_upload(eng._ctx, ctypes.byref(k), ctypes.byref(self.handle)), "keys_upload")
+        else:
+            eng._ck(eng.lib.tecdsa_keys_upload_parties(eng._ctx, self.parties, ctypes.byref(k), ctypes.byref(self.handle)), "keys_upload_parties")
 
     def table(self, index: int, limbs: int) -> List[int]:
-        out = np.zeros((self.n * 3, limbs), dtype=np.uint32)
+        out = np.zeros((self.n * self.parties, limbs), dtype=np.uint32)
         self.eng._ck(self.eng.lib.tecdsa_keys_table(self.eng._ctx, self.handle, index, out.ctypes.data), "keys_table")
         return limbs_to_ints(out)
 

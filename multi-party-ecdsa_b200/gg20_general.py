@@ -6,11 +6,12 @@ instances.  Element u = session * ttag + position; pair t = u * (ttag - 1) + j i
 No arithmetic happens on the host — only index bookkeeping and equality tests.  Oracle: oracle/gg20_general_oracle.py."""
 from __future__ import annotations
 
+import ctypes
 from typing import Dict, List, Optional, Sequence
 
 import numpy as np
 
-from . import SAMPLE_BELOW, SAMPLE_BITS, SAMPLE_RANGE1, SAMPLE_SCALAR, SAMPLE_UNIT, Engine, EngineError, limbs_to_ints
+from . import HOST, SAMPLE_BELOW, SAMPLE_BITS, SAMPLE_RANGE1, SAMPLE_SCALAR, SAMPLE_UNIT, Engine, EngineError, _ptr, ints_to_limbs, limbs_to_ints
 from . import gg18, gg20
 from .gg20 import KeySets, unpack_point
 
@@ -206,3 +207,150 @@ def offline_batch(eng: Engine, keys: KeySets, ttag: int, key_rows: Sequence[int]
             docs.append(m)
         out["messages"] = docs
     return out
+
+
+# ----------------------------------------------------------------------------- the one-call path (tecdsa_gg20_offline_general_batch)
+# widths (limbs) of the inputs: per element, per statement of MessageA's range proofs ([parties][E][w]), per pair ([signers-1][E][w])
+ELEMENT_FIELDS = {"gamma": 8, "k": 8, "blind": 8, "r_k": 64, "l": 8, "ped_s1": 8, "ped_s2": 8, "heg_s1": 8, "heg_s2": 8}
+STATEMENT_FIELDS = {"alice_alpha": 24, "alice_beta": 64, "alice_gamma": 88, "alice_rho": 72}
+PAIR_FIELDS = {"beta_tag_gamma": 64, "r_gamma": 64, "nonce_gamma_b": 8, "nonce_gamma_beta": 8, "beta_tag_w": 64, "r_w": 64, "nonce_w_b": 8,
+               "nonce_w_beta": 8, "pdl_alpha": 24, "pdl_beta": 64, "pdl_rho": 72, "pdl_gamma": 88}
+IN_FIELDS = list(ELEMENT_FIELDS) + list(STATEMENT_FIELDS) + list(PAIR_FIELDS)
+
+
+class _GeneralIn(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_void_p) for n in IN_FIELDS]
+
+
+class _GeneralOut(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_void_p) for n in ("status", "R", "sigma", "T", "complete")]
+
+
+def _descriptors(sessions, signers: int) -> np.ndarray:
+    """[n][1 + signers] uint32 on the host (a CUDA tensor is copied back: the descriptors are public)"""
+    from .keygen import _host
+    return np.ascontiguousarray(_host(sessions) if not isinstance(sessions, (list, tuple)) else np.asarray(sessions), dtype=np.uint32).reshape(-1, 1 + signers)
+
+
+def sample_inputs(eng: Engine, keys: KeySets, signers: int, sessions, seed: Optional[bytes] = None, mem: int = HOST) -> Dict[str, object]:
+    """Every input of `offline_device`, drawn by `tecdsa_sample_batch` on the stream and element ids `sample_rnd` uses, so the values
+    are the ones `sample_rnd` draws from the same seed: element u = session * signers + position has element id (sub << 32) | u,
+    sub = the statement x for the range-proof fields and the peer index j for the per-pair fields.  sessions = [n][1 + signers]
+    (key set, then s_l[p] - 1).  -> dict field -> array in the layout of tecdsa_offline_general_in (numpy for HOST; CUDA tensors for
+    DEVICE, which never reach the host).  seed=None draws a fresh seed; a seed serves ONE call."""
+    from .keygen import _buffer, _host, _upload
+    from . import seed_words
+    lib = eng.lib
+    if not getattr(lib, "_sample_bound", False):
+        V, S_, I_ = ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int
+        lib.tecdsa_sample_batch.argtypes = [V, V, ctypes.c_uint64, ctypes.c_uint32, I_, I_, V, V, S_, I_, V, V, S_, I_]
+        lib._sample_bound = True
+    d = _descriptors(sessions, signers)
+    T, P, n = signers, keys.parties, d.shape[0]
+    E, q = n * T, gg20._Q
+    # bound tables per key row (public key material) and the key row each element draws under
+    N, NT = keys.table(0, 64), keys.table(2, 64)
+    tabs = {"N": _upload(ints_to_limbs(N, 64), mem, eng.device), "QNT": _upload(ints_to_limbs([q * v for v in NT], 72), mem, eng.device),
+            "Q3NT": _upload(ints_to_limbs([q ** 3 * v for v in NT], 88), mem, eng.device), "Q3": _upload(ints_to_limbs([q ** 3], 24), mem, eng.device)}
+    own = (d[:, :1] * P + d[:, 1:]).reshape(E).astype(np.uint32)
+    pos = np.arange(E) % T
+    base = np.arange(E) - pos
+
+    def peer_rows(j):
+        return own[base + np.where(j < pos, j, j + 1)].astype(np.uint32)
+
+    sw = seed_words(gg20.fresh_seed(seed))
+
+    def draw(out, name, kind, stream, sub=0, tab=None, idx=None, bits=0):
+        limbs = out.shape[-1]
+        st = _buffer((E,), np.uint8, mem, eng.device)
+        ix = None if idx is None else _upload(np.asarray(idx, dtype=np.uint32), mem, eng.device)
+        nb = 0 if tab is None else tab.shape[0]
+        eng._ck(lib.tecdsa_sample_batch(eng._ctx, _ptr(sw), sub << 32, stream, kind, bits, _ptr(tab), _ptr(ix), nb, limbs, _ptr(out), _ptr(st), E, mem),
+                "sample_batch")
+        bad = np.flatnonzero(_host(st))
+        if bad.size:
+            raise EngineError(f"sampling {name}: element {int(bad[0])} has status {int(_host(st)[bad[0]])}")
+
+    inp = {f: _buffer((E, w), np.uint32, mem, eng.device) for f, w in ELEMENT_FIELDS.items()}
+    inp.update({f: _buffer((P, E, w), np.uint32, mem, eng.device) for f, w in STATEMENT_FIELDS.items()})
+    inp.update({f: _buffer((T - 1, E, w), np.uint32, mem, eng.device) for f, w in PAIR_FIELDS.items()})
+    zero = np.zeros(E, np.uint32)
+    A = gg20.RNDS_ALICE
+    try:
+        for f in ("gamma", "k", "l", "ped_s1", "ped_s2", "heg_s1", "heg_s2"):
+            draw(inp[f], f, SAMPLE_SCALAR, gg20.RNDS[f])
+        draw(inp["blind"], "blind", SAMPLE_BITS, gg20.RNDS["blind"], bits=256)
+        draw(inp["r_k"], "r_k", SAMPLE_BELOW, gg20.RNDS["r_k"], tab=tabs["N"], idx=own)
+        for x in range(P):
+            st_rows = (d[:, :1] * P + x).repeat(T, axis=1).reshape(E).astype(np.uint32)
+            draw(inp["alice_alpha"][x], "alice alpha", SAMPLE_BELOW, A, x, tabs["Q3"], zero)
+            draw(inp["alice_beta"][x], "alice beta", SAMPLE_UNIT, A + 1, x, tabs["N"], own)
+            draw(inp["alice_gamma"][x], "alice gamma", SAMPLE_BELOW, A + 2, x, tabs["Q3NT"], st_rows)
+            draw(inp["alice_rho"][x], "alice rho", SAMPLE_BELOW, A + 3, x, tabs["QNT"], st_rows)
+        for j in range(T - 1):
+            pr = peer_rows(j)
+            for f in ("beta_tag_gamma", "r_gamma", "beta_tag_w", "r_w"):
+                draw(inp[f][j], f, SAMPLE_BELOW, gg20.RNDS[f], j, tabs["N"], pr)
+            for f in ("nonce_gamma_b", "nonce_gamma_beta", "nonce_w_b", "nonce_w_beta"):
+                draw(inp[f][j], f, SAMPLE_SCALAR, gg20.RNDS[f], j)
+            draw(inp["pdl_alpha"][j], "pdl_alpha", SAMPLE_BELOW, gg20.RNDS["pdl_alpha"], j, tabs["Q3"], zero)
+            draw(inp["pdl_beta"][j], "pdl_beta", SAMPLE_RANGE1, gg20.RNDS["pdl_beta"], j, tabs["N"], own)
+            draw(inp["pdl_rho"][j], "pdl_rho", SAMPLE_BELOW, gg20.RNDS["pdl_rho"], j, tabs["QNT"], pr)
+            draw(inp["pdl_gamma"][j], "pdl_gamma", SAMPLE_BELOW, gg20.RNDS["pdl_gamma"], j, tabs["Q3NT"], pr)
+    finally:
+        sw[:] = 0
+    return inp
+
+
+def offline_device(eng: Engine, keys: KeySets, signers: int, sessions, inp: Dict[str, object], mem: int = HOST, out: Optional[Dict[str, object]] = None,
+                   check: bool = True) -> Dict[str, object]:
+    """`OfflineStage` Round0..Round6 for every session as ONE call (tecdsa_gg20_offline_general_batch).  sessions = [n][1 + signers];
+    inp = the dict `sample_inputs` returns (or the same fields from elsewhere).  -> dict(status [E], R [E][16], sigma [E][8],
+    T [E][16], complete [n]): numpy arrays for HOST, CUDA tensors for DEVICE (the caller's, when `out` holds them; sessions is then a
+    CUDA tensor too).  A session that did not complete has zero R, sigma and T.  check=False returns the call's rc instead of raising."""
+    from .keygen import _buffer
+    lib = eng.lib
+    if not getattr(lib, "_general_bound", False):
+        V = ctypes.c_void_p
+        lib.tecdsa_gg20_offline_general_batch.argtypes = [V, V, ctypes.c_int, ctypes.c_size_t, ctypes.c_int, V, ctypes.POINTER(_GeneralIn), ctypes.POINTER(_GeneralOut)]
+        lib._general_bound = True
+    if mem == HOST:
+        sessions = _descriptors(sessions, signers)
+        inp = {f: np.ascontiguousarray(v, dtype=np.uint32) for f, v in inp.items()}
+    n = sessions.shape[0]
+    E = n * signers
+    if out is None:
+        out = {"status": _buffer((E,), np.uint8, mem, eng.device), "R": _buffer((E, 16), np.uint32, mem, eng.device),
+               "sigma": _buffer((E, 8), np.uint32, mem, eng.device), "T": _buffer((E, 16), np.uint32, mem, eng.device),
+               "complete": _buffer((n,), np.uint8, mem, eng.device)}
+    gi = _GeneralIn(*[_ptr(inp[f]) for f in IN_FIELDS])
+    go = _GeneralOut(*[_ptr(out[f]) for f in ("status", "R", "sigma", "T", "complete")])
+    rc = lib.tecdsa_gg20_offline_general_batch(eng._ctx, keys.handle, signers, n, mem, _ptr(sessions), ctypes.byref(gi), ctypes.byref(go))
+    if not check:
+        return rc
+    eng._ck(rc, "gg20_offline_general_batch")
+    return out
+
+
+def sign_batch(eng: Engine, signers: int, message, R, sigma, k, y) -> Dict[str, np.ndarray]:
+    """GG20's online step (`phase7_local_sig` + `output_signature` + `verify`, party_i.rs:850-936) for completed sessions of
+    `signers` signers, on the existing GG18 entry points: s_i = m k_i + r sigma_i is `tecdsa_gg18_local_sig_batch`, and the sum with
+    low-s normalisation, recid and verification against y is `tecdsa_gg18_output_signature_batch` — the same arithmetic as GG18's
+    party_i.rs:486-730, so no entry point of its own is needed.  message [n] ints (reduced mod q), R [E][16], sigma [E][8], k [E][8]
+    (limb rows), y [n] points (y_sum_s).  -> dict(s_i [E][8], r [E][8], s [E][8], recid [E], status [E]) per element: every signer
+    derives the session's signature."""
+    from . import gg18
+    gg18._bind(eng.lib)
+    lib = eng.lib
+    R, sigma, k = (np.ascontiguousarray(a, dtype=np.uint32) for a in (R, sigma, k))
+    E = R.shape[0]
+    n = E // signers
+    msg = ints_to_limbs([int(message[u // signers]) for u in range(E)], 8)
+    Y = ints_to_limbs([gg20.pack_point(y[u // signers]) for u in range(E)], 16)
+    s_i, r, s = np.zeros((E, 8), np.uint32), np.zeros((E, 8), np.uint32), np.zeros((E, 8), np.uint32)
+    recid, status = np.zeros(E, np.uint8), np.full(E, 255, np.uint8)
+    eng._ck(lib.tecdsa_gg18_local_sig_batch(eng._ctx, _ptr(msg), _ptr(R), _ptr(k), _ptr(sigma), _ptr(s_i), E, HOST), "gg18_local_sig")
+    eng._ck(lib.tecdsa_gg18_output_signature_batch(eng._ctx, signers, _ptr(R), _ptr(Y), _ptr(msg), _ptr(s_i), _ptr(r), _ptr(s), _ptr(recid), _ptr(status), n, HOST),
+            "gg18_output_signature")
+    return {"s_i": s_i, "r": r, "s": s, "recid": recid, "status": status}
