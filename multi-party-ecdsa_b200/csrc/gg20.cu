@@ -404,8 +404,8 @@ static int offline_impl(tecdsa_ctx* c, const tecdsa_keyset* ks, const uint32_t* 
     // of the peer's MessageA are computed ONCE and used for both calls (declared de-duplication).
     RUN(glue(c, gg20_r1_pre, A));
     // (c^e)^-1 mod N^2 is evaluated as (c^-1)^e (the reference does the same in commitment_unknown_order,
-    // zk_pdl_with_slack/mod.rs:191-193): ONE inversion of the peer's ciphertext serves the three proofs here and the
-    // peer's PDL proof in round 5 (declared shortcut, identical value)
+    // zk_pdl_with_slack/mod.rs:191-193): ONE inversion of the peer's ciphertext serves the three proofs here (declared
+    // shortcut, identical value)
     B.inv_class(I128, GPWI128, B.key(KT_NN, rp), B.peer(F_CK), F_CINVP, 3);
     RUN(run_inv(c, I128, 128)); RUN(run_inv(c, B.I128H, -128));
     for (int x = 0; x < 3; x++)
@@ -437,7 +437,7 @@ static int offline_impl(tecdsa_ctx* c, const tecdsa_keyset* ks, const uint32_t* 
     RUN(glue(c, gg20_r2_check, A, 7));
     RUN(glue(c, gg20_r2_finish, A));
     // ================= Round 3 (rounds.rs:347-402)
-    RUN(glue(c, gg20_r3_check, A, 2));
+    RUN(glue(c, gg20_r3_check, A));
     RUN(glue(c, gg20_r3_finish, A));
     // ================= Round 4 (rounds.rs:431-498): R, R_dash, PDLwSlackProof::prove against the peer's statement
     RUN(glue(c, gg20_r4_pre, A));
@@ -456,39 +456,31 @@ static int offline_impl(tecdsa_ctx* c, const tecdsa_keyset* ks, const uint32_t* 
     B.exp_class(L64, GPW64, B.key(KT_N, ro), 1, B.rnd(RND_RK, 64), B.fld(F_PE), 8, NONE, NONE, 0, 1, B.rnd(RND_PDL_BETA, 64), NONE, F_PS2);   // s2 = r^e * beta mod N (:113)
     RUN(run_exp(c, B.LPQ, -32)); RUN(run_exp(c, L64, 64));
 
-    // ================= Round 5 (rounds.rs:525-592): verify both signers' PDL proofs (own one included)
+    // ================= Round 5 (rounds.rs:525-592): verify the PDL proofs.  Each unit verifies its own proof, as the reference's
+    // prover does; the peer's check of the same proof has the same inputs (R is bit-identical on both units), so the peer reads
+    // that verdict instead of running it again (declared shortcut 10)
     RUN(glue(c, gg20_r5_pre, A));
-    B.inv_class(I128, GPWI128, B.key(KT_NN, ro), B.fld(F_CK), F_CINVO, 8);          // own ciphertext (proof j = 0); the peer's inverse is CINVP
+    B.inv_class(I128, GPWI128, B.key(KT_NN, ro), B.fld(F_CK), F_CINVO, 8);          // own ciphertext
     RUN(run_inv(c, I128, 128)); RUN(run_inv(c, B.I128H, -128));
-    for (int j = 0; j < 2; j++) {
-        const uint32_t* stmt = j ? ro : rp;              // whose (N_tilde, h1, h2) the proof was made against
-        Operand z = j ? B.peer(F_PZ) : B.fld(F_PZ);
-        B.exp_class(L64, GPW64, B.key(KT_NT, stmt), 1, z, B.fld(F_VE0 + j), 8, NONE, NONE, 0, 0, NONE, NONE, F_VZE0 + j);       // z^e; (z^-1)^e == (z^e)^-1 (:166-172)
-    }
-    // (c^-1)^e (:151-157) of the own proof; the peer's proof takes it as the second base of its u2' job below
-    B.exp_class(L128, GPW128, B.key(KT_NN, ro), 1, B.fld(F_CINVO), B.fld(F_VE0), 8, NONE, NONE, 0, 0, NONE, NONE, F_VCEI0);
-    B.crt_stage1(L32, GPW32, ro, 5, B.fld(F_PS2, 64));       // own proof's s2^N mod N^2_own through the CRT stages
+    // z^e against the peer's (N_tilde, h1, h2), the statement the proof was made against; (z^-1)^e == (z^e)^-1 (:166-172)
+    B.exp_class(L64, GPW64, B.key(KT_NT, rp), 1, B.fld(F_PZ), B.fld(F_VE0), 8, NONE, NONE, 0, 0, NONE, NONE, F_VZE0);
+    B.exp_class(L128, GPW128, B.key(KT_NN, ro), 1, B.fld(F_CINVO), B.fld(F_VE0), 8, NONE, NONE, 0, 0, NONE, NONE, F_VCEI0);   // (c^-1)^e (:151-157)
+    B.crt_stage1(L32, GPW32, ro, 5, B.fld(F_PS2, 64));       // s2^N mod N^2_own through the CRT stages
     RUN(run_exp(c, L32, 32));
     B.crt_stage2(L64, GPW64, ro, 5);
     RUN(run_exp(c, L128, 128)); RUN(run_exp(c, B.LPQ, -32)); RUN(run_exp(c, L64, 64));
     RUN(glue_crt(c, A, 5, 1));
-    for (int j = 0; j < 2; j++) B.inv_class(I64, GPW64, B.key(KT_NT, j ? ro : rp), B.fld(F_VZE0 + j), F_VZEI0 + j, 6 + j);
+    B.inv_class(I64, GPW64, B.key(KT_NT, rp), B.fld(F_VZE0), F_VZEI0, 6);
     RUN(run_inv(c, I64, 64));
-    for (int j = 0; j < 2; j++) {
-        const uint32_t* prover = j ? rp : ro;            // key row of the prover
-        const uint32_t* stmt = j ? ro : rp;
-        Operand s1 = j ? B.peer(F_PS1) : B.fld(F_PS1), s2 = j ? B.peer(F_PS2, 64) : B.fld(F_PS2, 64), s3 = j ? B.peer(F_PS3) : B.fld(F_PS3);
-        // u3' = h1^s1 * h2^s3 * z^-e mod N_tilde                         (:158-172)
-        B.fb_class(L64, GPW64, stmt, s3, 92, s1, 28, 1, B.fld(F_VZEI0 + j), F_VU30 + j);
-        // u2' = (N+1)^s1 * s2^N * c^-e mod N^2                           (:144-157)
-        if (j == 0) B.exp_class(L128, GPW128, B.key(KT_NN, prover), 0, NONE, NONE, 0, NONE, NONE, 0, 3, B.fld(F_VLIN0), B.fld(F_VCEI0), F_VU20, 0, B.fld(F_XC5));
-        else B.exp_class(L128, GPW128, B.key(KT_NN, prover), 2, s2, B.key(KT_N, prover), 64, B.fld(F_CINVP), B.fld(F_VE1), 8, 1, B.fld(F_VLIN1), NONE, F_VU21);
-    }
+    // u3' = h1^s1 * h2^s3 * z^-e mod N_tilde                             (:158-172)
+    B.fb_class(L64, GPW64, rp, B.fld(F_PS3), 92, B.fld(F_PS1), 28, 1, B.fld(F_VZEI0), F_VU30);
+    // u2' = (N+1)^s1 * s2^N * c^-e mod N^2                               (:144-157)
+    B.exp_class(L128, GPW128, B.key(KT_NN, ro), 0, NONE, NONE, 0, NONE, NONE, 0, 3, B.fld(F_VLIN0), B.fld(F_VCEI0), F_VU20, 0, B.fld(F_XC5));
     RUN(run_exp(c, L128, 128)); RUN(run_exp(c, B.LPQ, -32)); RUN(run_exp(c, L64, 64));
-    RUN(glue(c, gg20_r5_check, A, 2));
+    RUN(glue(c, gg20_r5_check, A));
     RUN(glue(c, gg20_r5_finish, A));
     // ================= Round 6 (rounds.rs:612-636) + result records
-    RUN(glue(c, gg20_r6_check, A, 2));
+    RUN(glue(c, gg20_r6_check, A));
     RUN(glue(c, gg20_r6, A));
 #undef RUN
     CK(cudaEventRecord(c->ev1, c->stream));
@@ -568,6 +560,7 @@ int tecdsa_internal_offline(tecdsa_ctx* c, const tecdsa_keyset* ks, const uint32
     std::string errs[2];
     auto half = [&](int h) {
         tecdsa_ctx* cc = c->child[h];
+        // halves are cut on session boundaries: a unit's peer, whose proof verdicts it reads, is always in the same arena
         const size_t s0 = h ? n0 : 0, ns = h ? n_sessions - n0 : n0, u0 = 2 * s0;
         cudaSetDevice(cc->device);
         cudaError_t e = cudaStreamWaitEvent(cc->stream, c->ev_fork, 0);

@@ -46,9 +46,8 @@ enum : int {
     /* round 4 */                                                                                 \
     X(R, 16) X(RD, 16) X(PZ, 64) X(PU1, 16) X(PU2, 128) X(PU3, 64) X(PLIN, 128)                   \
     X(PE, 8) X(PS1, 28) X(PS2, 64) X(PS3, 92)                                                     \
-    /* round 5: j = 0 own proof, j = 1 the peer's proof */                                        \
-    X(VE0, 8) X(VE1, 8) X(VLIN0, 128) X(VLIN1, 128) X(VZE0, 64) X(VZE1, 64) \
-    X(VZEI0, 64) X(VZEI1, 64) X(VCEI0, 128) X(VU20, 128) X(VU21, 128) X(VU30, 64) X(VU31, 64) \
+    /* round 5: verification of the unit's own proof (the peer verifies its own on its unit) */   \
+    X(VE0, 8) X(VLIN0, 128) X(VZE0, 64) X(VZEI0, 64) X(VCEI0, 128) X(VU20, 128) X(VU30, 64)        \
     X(SI, 16) X(HEG, 48)                            /* T 16 | A3 16 | z1 8 | z2 8 */             \
     X(DIGEST, 8)                                                                                  \
     X(FLAGS, 8)                                     /* one ok byte per check, see gg20_glue.cuh */          \

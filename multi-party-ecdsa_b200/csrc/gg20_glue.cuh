@@ -39,8 +39,9 @@ struct Arena {
     __device__ __forceinline__ uint8_t* flags(int u) const { return reinterpret_cast<uint8_t*>(p(F_FLAGS, u)); }
     __device__ __forceinline__ void fail(int u, uint8_t code) const { if (status[u] == 0) status[u] = code; }
 };
-// FLAGS bytes: 0..2 ZEI ok, 3 peer ciphertext invertible, 6..7 VZEI ok, 8 own ciphertext invertible, 10 range bits, 11..12 MessageB checks ok,
-// 13 g_w_vec ok, 14..15 Pedersen ok, 16..17 PDL ok, 18..19 HomoElGamal ok, 20..22 AliceProof challenge ok, 24..27 MessageB DLogProofs ok
+// FLAGS bytes: 0..2 ZEI ok, 3 peer ciphertext invertible, 6 VZEI ok, 8 own ciphertext invertible, 10 range bits, 11..12 MessageB checks ok,
+// 13 g_w_vec ok, 14 Pedersen ok, 16 PDL ok, 18 HomoElGamal ok (of the unit's own proof; the peer's finish kernels read it there),
+// 20..22 AliceProof challenge ok, 24..27 MessageB DLogProofs ok.  Bytes 7, 15, 17 and 19 are not written.
 
 // ------------------------------------------------------------------------------ small helpers
 __device__ __forceinline__ U256 load_scalar(const uint32_t* p) { return sc_reduce_once(u256_load(p), 0); }

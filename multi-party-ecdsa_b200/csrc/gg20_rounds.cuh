@@ -150,20 +150,20 @@ static __global__ void gg20_r2_finish(Arena A) {
     u256_store(ped + 40, sc_add(s1, sc_mul(e, sigma))); u256_store(ped + 48, sc_add(s2, sc_mul(e, l)));
 }
 
-// one thread per (unit, signer): PedersenProof::verify of the own (j = 0) and the peer's (j = 1) proof
+// PedersenProof::verify of the unit's own proof.  Both signers of a session check every proof of the session on the same inputs
+// (no input comes from the verifier's side), so each proof is checked once, on its prover's unit, and the peer's finish kernel
+// reads that verdict (declared shortcut 10, DESIGN.md section 4).  The same holds for the PDL and HomoElGamal checks below.
 static __global__ void gg20_r3_check(Arena A) {
-    int t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= A.U * 2) return;
-    const int u = t >> 1, j = t & 1, src = j ? A.peer[u] : u;
-    A.flags(u)[14 + j] = pedersen_verify(A.p(F_PED, src), affine_load(A.p(F_T, src)));
+    int u = blockIdx.x * blockDim.x + threadIdx.x;
+    if (u >= A.U) return;
+    A.flags(u)[14] = pedersen_verify(A.p(F_PED, u), affine_load(A.p(F_T, u)));
 }
 
 static __global__ void gg20_r3_finish(Arena A) {
     int u = blockIdx.x * blockDim.x + threadIdx.x;
     if (u >= A.U) return;
     const int pu = A.peer[u];
-    const uint8_t* fl = A.flags(u);
-    if (!(fl[14] && fl[15])) A.fail(u, TECDSA_ST_PROOF);
+    if (!(A.flags(u)[14] && A.flags(pu)[14])) A.fail(u, TECDSA_ST_PROOF);
     U256 sum = sc_add(u256_load(A.p(F_DELTA, u)), u256_load(A.p(F_DELTA, pu)));
     if (u256_is_zero(sum)) A.fail(u, TECDSA_ST_PROOF);          // reference: .unwrap() panic on a zero sum
     u256_store(A.p(F_DINV, u), sc_inv(sum));
@@ -182,6 +182,9 @@ static __global__ void gg20_r4_pre(Arena A) {
     hash_commit_point(com, gg_peer, A.p(F_RND, pu) + RND_BLIND);
     bool ok = affine_eq(affine_load(A.p(F_DL0, pu)), gg_peer) && st::cmp(com, A.p(F_COM, pu), 8) == 0;
     if (!ok) A.fail(u, TECDSA_ST_COMMITMENT);
+    // R is bit-identical on the two units of a session, which lets one unit's PDL and HomoElGamal verdicts stand for both: the
+    // operand order of the sum and the per-unit k and alpha change only the projective representation and the other two
+    // outputs of the shared inversion, and the affine R is the unique (X/Z^2, Y/Z^3) or the identity (tests/test_session_verdicts.py)
     const Jac Rj = jac_mul(j_add_aff(gg_own, gg_peer), u256_load(A.p(F_DINV, u)));
     // R_dash and u1 are multiples of R: they are computed from the projective R and all three are normalised together
     Affine R, Rd, U1;
@@ -205,37 +208,32 @@ static __global__ void gg20_r4_mid(Arena A) {
 }
 
 // ------------------------------------------------------------------------------ round 5
-// PDLwSlackProof::verify for both signers' proofs (party_i.rs:719-766 -> zk_pdl_with_slack/mod.rs:127-179)
+// PDLwSlackProof::verify of the unit's own proof (party_i.rs:719-766 -> zk_pdl_with_slack/mod.rs:127-179), the check the
+// reference runs on the prover's side (sign/rounds.rs:546-558).  Its one verifier-side input, R, is bit-identical on the two
+// units of a session (gg20_r4_pre), so the verdict is the peer's verdict on this proof too.
 static __global__ void gg20_r5_pre(Arena A) {
     int u = blockIdx.x * blockDim.x + threadIdx.x;
     if (u >= A.U) return;
-    const int pu = A.peer[u];
-    Affine R = affine_load(A.p(F_R, u));
     uint32_t one = 1;
-    for (int j = 0; j < 2; j++) {
-        const int src = j ? pu : u;
-        const uint32_t prow = j ? A.row_peer[u] : A.row_own[u];
-        pdl_hash(A.p(F_VE0 + j, u), R, affine_load(A.p(F_RD, src)), A.p(F_CK, src), A.p(F_PZ, src), affine_load(A.p(F_PU1, src)),
-                 A.p(F_PU2, src), A.p(F_PU3, src));
-        st::mul_add(A.p(F_VLIN0 + j, u), 128, A.p(F_PS1, src), 28, A.k(KT_N, prow), 64, &one, 1);
-    }
+    pdl_hash(A.p(F_VE0, u), affine_load(A.p(F_R, u)), affine_load(A.p(F_RD, u)), A.p(F_CK, u), A.p(F_PZ, u), affine_load(A.p(F_PU1, u)),
+             A.p(F_PU2, u), A.p(F_PU3, u));
+    st::mul_add(A.p(F_VLIN0, u), 128, A.p(F_PS1, u), 28, A.k(KT_N, A.row_own[u]), 64, &one, 1);
 }
 
-// one thread per (unit, proof): the EC relation and the two big-integer comparisons of PDLwSlackProof::verify
+// the EC relation and the two big-integer comparisons of PDLwSlackProof::verify
 static __global__ void gg20_r5_check(Arena A) {
-    int t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= A.U * 2) return;
-    const int u = t >> 1, j = t & 1, src = j ? A.peer[u] : u;
+    int u = blockIdx.x * blockDim.x + threadIdx.x;
+    if (u >= A.U) return;
     const uint8_t* fl = A.flags(u);
     Affine R = affine_load(A.p(F_R, u));
-    U256 e = sc_from_limbs(A.p(F_VE0 + j, u), 8);
-    U256 s1 = sc_from_limbs(A.p(F_PS1, src), 28);
-    const Jac u1t = j_lin2(R, s1, affine_load(A.p(F_RD, src)), sc_neg(e));
-    bool ok = fl[6 + j] && (j ? fl[3] : fl[8]);       // z and the prover's ciphertext invertible
-    ok = ok && jac_eq_affine(u1t, affine_load(A.p(F_PU1, src)));
-    ok = ok && st::cmp(A.p(F_VU20 + j, u), A.p(F_PU2, src), 128) == 0;
-    ok = ok && st::cmp(A.p(F_VU30 + j, u), A.p(F_PU3, src), 64) == 0;
-    A.flags(u)[16 + j] = ok;
+    U256 e = sc_from_limbs(A.p(F_VE0, u), 8);
+    U256 s1 = sc_from_limbs(A.p(F_PS1, u), 28);
+    const Jac u1t = j_lin2(R, s1, affine_load(A.p(F_RD, u)), sc_neg(e));
+    bool ok = fl[6] && fl[8];                         // z^e mod N_tilde and the prover's ciphertext mod N^2 invertible
+    ok = ok && jac_eq_affine(u1t, affine_load(A.p(F_PU1, u)));
+    ok = ok && st::cmp(A.p(F_VU20, u), A.p(F_PU2, u), 128) == 0;
+    ok = ok && st::cmp(A.p(F_VU30, u), A.p(F_PU3, u), 64) == 0;
+    A.flags(u)[16] = ok;
 }
 
 static __global__ void gg20_r5_finish(Arena A) {
@@ -243,9 +241,8 @@ static __global__ void gg20_r5_finish(Arena A) {
     if (u >= A.U) return;
     const int pu = A.peer[u];
     const uint32_t* rnd = A.p(F_RND, u);
-    const uint8_t* fl = A.flags(u);
     Affine R = affine_load(A.p(F_R, u));
-    if (!(fl[16] && fl[17])) A.fail(u, TECDSA_ST_PDL_VERIFY);
+    if (!(A.flags(u)[16] && A.flags(pu)[16])) A.fail(u, TECDSA_ST_PDL_VERIFY);
     // phase5_check_R_dash_sum (party_i.rs:768-776): G + sum(R_dash) - G == G
     if (!jac_eq_affine(j_add_aff(affine_load(A.p(F_RD, u)), affine_load(A.p(F_RD, pu))), affine_G())) A.fail(u, TECDSA_ST_PHASE5_BAD_SUM);
     // phase6_compute_S_i_and_proof_of_consistency (party_i.rs:778-799)
@@ -266,20 +263,18 @@ static __global__ void gg20_r5_finish(Arena A) {
 
 // phase6_verify_proof + phase6_check_S_i_sum (party_i.rs:801-848), then the unit's result record:
 // a SHA-256 over every message it emitted, in the fixed-width encoding of oracle/gg20_oracle.py
-// one thread per (unit, signer): HomoELGamalProof::verify (party_i.rs:801-833)
+// HomoELGamalProof::verify of the unit's own proof (party_i.rs:801-833); R is the session's R, bit-identical on both units
 static __global__ void gg20_r6_check(Arena A) {
-    int t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= A.U * 2) return;
-    const int u = t >> 1, j = t & 1, src = j ? A.peer[u] : u;
-    A.flags(u)[18 + j] = heg_verify(A.p(F_HEG, src), affine_load(A.p(F_R, u)), affine_load(A.p(F_T, src)), affine_load(A.p(F_SI, src)));
+    int u = blockIdx.x * blockDim.x + threadIdx.x;
+    if (u >= A.U) return;
+    A.flags(u)[18] = heg_verify(A.p(F_HEG, u), affine_load(A.p(F_R, u)), affine_load(A.p(F_T, u)), affine_load(A.p(F_SI, u)));
 }
 
 static __global__ void gg20_r6(Arena A) {
     int u = blockIdx.x * blockDim.x + threadIdx.x;
     if (u >= A.U) return;
     const int pu = A.peer[u];
-    const uint8_t* fl = A.flags(u);
-    if (!(fl[18] && fl[19])) A.fail(u, TECDSA_ST_PHASE6);
+    if (!(A.flags(u)[18] && A.flags(pu)[18])) A.fail(u, TECDSA_ST_PHASE6);
     if (!jac_eq_affine(j_add_aff(affine_load(A.p(F_SI, u)), affine_load(A.p(F_SI, pu))), affine_load(A.ypk + (size_t)A.keyset[u] * 16))) A.fail(u, TECDSA_ST_PHASE6);
 
     Sha256 h; h.init();
