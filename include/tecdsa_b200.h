@@ -413,6 +413,65 @@ int tecdsa_gg18_phase5d_batch(tecdsa_ctx* ctx, int parties, const uint32_t* deco
 int tecdsa_gg18_output_signature_batch(tecdsa_ctx* ctx, int parties, const uint32_t* R, const uint32_t* y, const uint32_t* message,
                                        const uint32_t* s_i, uint32_t* sig_r, uint32_t* sig_s, uint8_t* recid, uint8_t* status,
                                        size_t sessions, int mem);
+/* ---- GG18 signing as one call: phases 1-5, `output_signature` and `verify` (gg_2018/test.rs `sign` :163-403, party_i.rs:385-730)
+ * for `n_sessions` sessions of `signers` signers of keys in ks (key sets of 2..64 parties, tecdsa_keys_upload_parties).
+ * sessions = [n_sessions][1 + signers] and the element layout are those of tecdsa_gg20_offline_general_batch: the key set, then
+ * s_l[p] - 1 of every signer position p; element u = s*signers + p; per-pair inputs [signers-1][E] peer-major (slab j holds element
+ * u towards its j-th peer, position j < p ? j : j + 1).  message = [n_sessions][8], the hashed message reduced mod q.  A key set
+ * out of range, a signer index out of range or repeated, signers < 2 or > parties, n_sessions > 2^24 or
+ * n_sessions * signers * parties > 2^26, a NULL buffer or a bad mem fails the whole call with TECDSA_E_ARG before anything is
+ * touched; n_sessions = 0 returns 0.  The call reads the Paillier rows (N, N^2, p^2, q^2, the CRT constants), x_i, pk and y of the
+ * key set, never its N~ / h1 / h2 rows.  w_i = lambda_i x_i is computed on the device from s_l (SignKeys::create).
+ * Flow: phase 1 g^gamma_i, its commitment and MessageA = Enc(k_i) (no range proofs: MessageA::a(&k_i, &ek, &[])); phase 2 the
+ * 2*(signers-1)*E MessageB::b (gamma_i and w_i towards every peer, under the peer's key) as one batch, then every
+ * verify_proofs_get_alpha; delta_i, sigma_i; phase 3 the session's delta^-1; phase 4 the decommitments and R; phase 5 s_i, 5a/5b,
+ * 5c, 5d, then output_signature with the in-tree verify.
+ * Status per element = the first error of its own phase:
+ *   MessageB::b fails          the sender, with the step's code;
+ *   verify_proofs_get_alpha    the receiver, TECDSA_ST_INVALID_KEY;
+ *   phase 3                    every member when the session's delta sum is 0, TECDSA_ST_NOT_INVERTIBLE;
+ *   phase 4                    a bad decommitment or MessageB(gamma) key, TECDSA_ST_INVALID_KEY;
+ *   phase 5a                   an identity point (a zero l, rho, nonce), TECDSA_ST_INVALID_KEY;
+ *   phase 5c / 5d              as tecdsa_gg18_phase5c_batch / _phase5d_batch;
+ *   output                     `verify` rejects the signature, TECDSA_ST_INVALID_SIG.
+ * A session stops at the first phase in which any member failed: members that did not fail keep TECDSA_ST_OK, later phases are not
+ * recorded, its R and signature are zero and complete = 0.  Every intermediate lives in stage scratch wiped before the call returns.
+ * Declared work-saving identity, value-preserving: in phase 5c every signer checks every other signer's 5a message (the commitment
+ * reopens, the HomoElGamal proof and the DLogProof of rho hold).  Those checks are deterministic in the sender's message and R, and
+ * R is the same on every member of a session that passed phase 4 (phase 4 derives it from session-wide values; otherwise the
+ * session has stopped), so each sender's message is checked once: signers HomoElGamal and DLog verifications per session instead
+ * of signers * (signers - 1).  mem = TECDSA_HOST or TECDSA_DEVICE for every buffer; sessions is read through a host copy.      */
+typedef struct {
+    const uint32_t* k;                /* [E][8]    k_i (SCALAR, party_i.rs:396-402)                        */
+    const uint32_t* gamma;            /* [E][8]    gamma_i (SCALAR)                                       */
+    const uint32_t* blind;            /* [E][8]    phase-1 commitment blind (BITS 256, :409)              */
+    const uint32_t* r_a;              /* [E][64]   Paillier randomness of MessageA (BELOW N_own, mta/mod.rs:57) */
+    const uint32_t* l;                /* [E][8]    l_i (SCALAR, :501-502)                                 */
+    const uint32_t* rho;              /* [E][8]    rho_i (SCALAR)                                         */
+    const uint32_t* blind5;           /* [E][8]    phase-5a commitment blind (BITS 256, :521)             */
+    const uint32_t* blind5c;          /* [E][8]    phase-5c commitment blind (BITS 256, :616)             */
+    const uint32_t* heg_s1;           /* [E][8]    HomoELGamalProof nonces (SCALAR)                       */
+    const uint32_t* heg_s2;           /* [E][8]                                                          */
+    const uint32_t* dlog_nonce;       /* [E][8]    nonce of the DLogProof of rho (SCALAR)                 */
+    const uint32_t* beta_tag_gamma;   /* [signers-1][E][64]  BELOW N_peer (mta/mod.rs:97-98)              */
+    const uint32_t* r_gamma;          /* [signers-1][E][64]  BELOW N_peer                                 */
+    const uint32_t* beta_tag_w;       /* [signers-1][E][64]                                               */
+    const uint32_t* r_w;              /* [signers-1][E][64]                                               */
+    const uint32_t* nonce_gamma_b;    /* [signers-1][E][8]   DLogProof nonces of the two MessageB (SCALAR, :147-148) */
+    const uint32_t* nonce_gamma_beta; /* [signers-1][E][8]                                                */
+    const uint32_t* nonce_w_b;        /* [signers-1][E][8]                                                */
+    const uint32_t* nonce_w_beta;     /* [signers-1][E][8]                                                */
+} tecdsa_gg18_signing_in;
+typedef struct {
+    uint8_t* status;                  /* [E]                                                             */
+    uint32_t* R;                      /* [E][16]                                                         */
+    uint32_t* sig_r;                  /* [n_sessions][8]                                                 */
+    uint32_t* sig_s;                  /* [n_sessions][8]   low-s normalised                              */
+    uint8_t* recid;                   /* [n_sessions]                                                    */
+    uint8_t* complete;                /* [n_sessions]  1 = every member finished and the signature verifies */
+} tecdsa_gg18_signing_out;
+int tecdsa_gg18_signing_batch(tecdsa_ctx* ctx, const tecdsa_keyset* ks, int signers, size_t n_sessions, int mem, const uint32_t* sessions,
+                              const uint32_t* message, const tecdsa_gg18_signing_in* in, const tecdsa_gg18_signing_out* out);
 
 /* ---- L3: the batched GG20 offline-signing stage ----------------------------------------
  * One "unit" = one party's OfflineStage Round0..Round6
@@ -621,6 +680,16 @@ enum {
 enum {
     TECDSA_RNDS_KG_U = 64, TECDSA_RNDS_KG_COEFF = 65, TECDSA_RNDS_KG_BLIND = 66, TECDSA_RNDS_KG_H1 = 67, TECDSA_RNDS_KG_XHI = 68,
     TECDSA_RNDS_KG_CDL = 69, TECDSA_RNDS_KG_DLOG = 70
+};
+/* Stream ids of the inputs of tecdsa_gg18_signing_batch, disjoint from the two sets above.  Element id = (sub << 32) | u for
+ * element u of the call: sub = 0 for the per-element fields, the peer index j for the per-pair fields of slab j.  Kinds as in
+ * tecdsa_gg18_signing_in: the blinds BITS(256), r_a BELOW(N_own), beta' and r' BELOW(N_peer), everything else SCALAR.            */
+enum {
+    TECDSA_RNDS_G18_K = 80, TECDSA_RNDS_G18_GAMMA = 81, TECDSA_RNDS_G18_BLIND = 82, TECDSA_RNDS_G18_R_A = 83, TECDSA_RNDS_G18_L = 84,
+    TECDSA_RNDS_G18_RHO = 85, TECDSA_RNDS_G18_BLIND5 = 86, TECDSA_RNDS_G18_BLIND5C = 87, TECDSA_RNDS_G18_HEG_S1 = 88,
+    TECDSA_RNDS_G18_HEG_S2 = 89, TECDSA_RNDS_G18_DLOG_NONCE = 90, TECDSA_RNDS_G18_BETATAG_GAMMA = 91, TECDSA_RNDS_G18_R_GAMMA = 92,
+    TECDSA_RNDS_G18_BETATAG_W = 93, TECDSA_RNDS_G18_R_W = 94, TECDSA_RNDS_G18_NONCE_GAMMA_B = 95, TECDSA_RNDS_G18_NONCE_GAMMA_BETA = 96,
+    TECDSA_RNDS_G18_NONCE_W_B = 97, TECDSA_RNDS_G18_NONCE_W_BETA = 98
 };
 /* rnd = [2*n_sessions][TECDSA_RND_LIMBS], the record tecdsa_gg20_offline_batch reads, every field drawn as the reference draws
  * it: scalars SCALAR, the blind BITS(256), r_k BELOW(N_own), per statement x alpha BELOW(q^3), beta UNIT(N_own), gamma

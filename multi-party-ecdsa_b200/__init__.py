@@ -54,7 +54,7 @@ EXPORTS = [
     "tecdsa_gg18_phase4_batch", "tecdsa_gg18_local_sig_batch", "tecdsa_gg18_phase5a_batch", "tecdsa_gg18_phase5c_batch", "tecdsa_gg18_phase5d_batch",
     "tecdsa_gg18_output_signature_batch",
     "tecdsa_sample_batch", "tecdsa_gg20_sample_randomness", "tecdsa_gg20_keygen_batch",
-    "tecdsa_keys_upload_parties", "tecdsa_gg20_offline_general_batch",
+    "tecdsa_keys_upload_parties", "tecdsa_gg20_offline_general_batch", "tecdsa_gg18_signing_batch",
 ]
 
 

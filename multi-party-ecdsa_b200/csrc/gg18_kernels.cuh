@@ -99,10 +99,34 @@ __device__ __noinline__ bool heg_verify_general(const uint32_t* heg, const Affin
     return ok1 && ok2;
 }
 
+// ---- phase 5c's checks of one sender's 5a message, run once per sender (party_i.rs:580-600): its commitment reopens to
+// (V, A, B), its HomoELGamalProof holds for (G = A, H = R, Y = g, D = V, E = B) and its DLogProof of rho holds.  verdict[v] = 1
+// when all three hold.  Each check is deterministic in the sender's message and R; R is the same on every member of a session that
+// passed phase 4 (k_gg18_phase4 derives it from session-wide values), so the sender's own R stands for every receiver's.
+__global__ void k_gg18_phase5c_senders(const uint32_t* R16, const uint32_t* com8, const uint32_t* vab48, const uint32_t* blind1, const uint32_t* heg48,
+                                       const uint32_t* dlog40, uint8_t* verdict, int count) {
+    int v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= count) return;
+    const uint32_t* d = vab48 + (size_t)v * 48;
+    Affine pts[3];
+    pts[0] = affine_load(d); pts[1] = affine_load(d + 16); pts[2] = affine_load(d + 32);
+    bool ok = good_point(pts[0]) && good_point(pts[1]) && good_point(pts[2]);
+    if (ok) {
+        uint32_t t[8];
+        commit_points(t, pts, 3, blind1 + (size_t)v * 8);
+        ok = limbs_eq8(t, com8 + (size_t)v * 8) && heg_verify_general(heg48 + (size_t)v * 48, pts[1], affine_load(R16 + (size_t)v * 16), pts[0], pts[2]) &&
+             dlog_verify(dlog40 + (size_t)v * 40);
+    }
+    verdict[v] = ok ? 1 : 0;
+}
+
 // ---- phase 5c (party_i.rs:560-629) ------------------------------------------------------------------------------------
+// sender_ok = NULL: every element checks every other signer's 5a message itself.  Otherwise sender_ok[v] is the verdict of
+// k_gg18_phase5c_senders for element v, read in place of the three checks (same com2, decom2 and status when R is the same on
+// every member of the session).
 __global__ void k_gg18_phase5c(int parties, const uint32_t* R16, const uint32_t* y16, const uint32_t* msg8, const uint32_t* rho8, const uint32_t* l8,
                                const uint32_t* blind2, const uint32_t* com8, const uint32_t* vab48, const uint32_t* blind1, const uint32_t* heg48,
-                               const uint32_t* dlog40, uint32_t* com2, uint32_t* ut32, uint8_t* status, int count) {
+                               const uint32_t* dlog40, uint32_t* com2, uint32_t* ut32, uint8_t* status, int count, const uint8_t* sender_ok = nullptr) {
     int u = blockIdx.x * blockDim.x + threadIdx.x;
     if (u >= count) return;
     const int s0 = (u / parties) * parties;
@@ -118,6 +142,10 @@ __global__ void k_gg18_phase5c(int parties, const uint32_t* R16, const uint32_t*
         vsum = jac_madd(vsum, pts[0]);
         if (v == u) continue;                                     // own V_i joins the sum; only the others' messages are checked
         asum = jac_madd(asum, pts[1]);
+        if (sender_ok) {
+            if (!sender_ok[v]) ok = false;
+            continue;
+        }
         uint32_t t[8];
         commit_points(t, pts, 3, blind1 + (size_t)v * 8);
         if (!limbs_eq8(t, com8 + (size_t)v * 8)) ok = false;

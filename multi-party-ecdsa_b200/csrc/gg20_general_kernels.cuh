@@ -4,26 +4,14 @@
 // Element u = s * T + p is signer position p of session s (T signers); pair j * E + u (E = elements, NP = (T - 1) * E pairs) is
 // "element u towards its j-th peer", the peer being position ind(p, j) = j < p ? j : j + 1 of the same session.  Round-1 / round-2
 // batches hold two halves, h * NP + pair: h = 0 for MessageB(gamma_i), h = 1 for MessageB(w_i).
-// sess = [sessions][1 + T]: the key set, then the keygen index - 1 of every signer position.
+// sess = [sessions][1 + T]: the key set, then the keygen index - 1 of every signer position.  The index helpers (peer_of,
+// pair_to, key_row) are in signing_layout.cuh, shared with the GG18 signing call.
 // Device code only (no runtime calls), so that tests/host_harness compiles it for the CPU.
 #pragma once
-#include "gg20_glue.cuh"
+#include "signing_layout.cuh"
 
 namespace tecdsa {
 namespace gen {
-
-__device__ __forceinline__ int peer_of(int T, int u, int j) { const int p = u % T; return u - p + (j < p ? j : j + 1); }
-// the pair in which element b sends to element v of the same session
-__device__ __forceinline__ int pair_to(int T, int E, int b, int v) { const int pb = b % T, pv = v % T; return (pv < pb ? pv : pv - 1) * E + b; }
-__device__ __forceinline__ uint32_t key_row(const uint32_t* sess, int T, int P, int u) {
-    const uint32_t* d = sess + (size_t)(u / T) * (1 + T);
-    return d[0] * (uint32_t)P + d[1 + u % T];
-}
-__device__ __forceinline__ bool eq16(const uint32_t* a, const uint32_t* b) {
-    uint32_t x = 0;
-    for (int i = 0; i < 16; i++) x |= a[i] ^ b[i];
-    return x == 0;
-}
 
 // Index tables of a call, one thread per entry (threads = max(P, 2 (T - 1)) * E):
 //   row[E]            key row of element u;

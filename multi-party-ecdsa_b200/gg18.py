@@ -231,3 +231,112 @@ def keygen_batch(eng: Engine, t: int, n: int, u, p_q, blind, polynomials, dlog_n
         if dv[sess(e):sess(e) + n].any() and not status[e]:
             status[e] = 2                                         # verify_dlog_proofs -> Err(InvalidKey)
     return {"status": status, "y": y, "x_i": x_i, "y_i": y_i, "com": com, "correct_key_proof": sigma, "commitments": commitments, "shares": shares, "dlog": dlog}
+
+
+# ----------------------------------------------------------------------------- signing as one call (tecdsa_gg18_signing_batch)
+# widths (limbs) of the inputs: per element ([E][w]) and per pair ([signers-1][E][w], slab j = element u towards its j-th peer)
+ELEMENT_FIELDS = {"k": 8, "gamma": 8, "blind": 8, "r_a": 64, "l": 8, "rho": 8, "blind5": 8, "blind5c": 8, "heg_s1": 8, "heg_s2": 8, "dlog_nonce": 8}
+PAIR_FIELDS = {"beta_tag_gamma": 64, "r_gamma": 64, "beta_tag_w": 64, "r_w": 64, "nonce_gamma_b": 8, "nonce_gamma_beta": 8, "nonce_w_b": 8, "nonce_w_beta": 8}
+IN_FIELDS = list(ELEMENT_FIELDS) + list(PAIR_FIELDS)
+OUT_FIELDS = ("status", "R", "sig_r", "sig_s", "recid", "complete")
+# TECDSA_RNDS_G18_*: one stream per field, in the order of tecdsa_gg18_signing_in
+RNDS = {f: 80 + i for i, f in enumerate(IN_FIELDS)}
+
+
+class _SigningIn(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_void_p) for n in IN_FIELDS]
+
+
+class _SigningOut(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_void_p) for n in OUT_FIELDS]
+
+
+def _descriptors(sessions, signers: int) -> np.ndarray:
+    """[n][1 + signers] uint32 on the host (a CUDA tensor is copied back: the descriptors are public)"""
+    from .keygen import _host
+    return np.ascontiguousarray(_host(sessions) if not isinstance(sessions, (list, tuple)) else np.asarray(sessions), dtype=np.uint32).reshape(-1, 1 + signers)
+
+
+def sample_inputs(eng: Engine, keys, signers: int, sessions, seed=None, mem: int = HOST):
+    """Every input of `sign_device`, drawn by `tecdsa_sample_batch` as the reference draws it (kinds in tecdsa_gg18_signing_in) on
+    the TECDSA_RNDS_G18_* streams.  Element u = session * signers + position has element id (sub << 32) | u, sub = 0 for the
+    per-element fields and the peer index j for the per-pair fields (the rule of the key-generation streams).  keys = gg20.KeySets;
+    sessions = [n][1 + signers] (key set, then s_l[p] - 1).  -> dict field -> array in the layout of tecdsa_gg18_signing_in (numpy
+    for HOST; CUDA tensors for DEVICE, which never reach the host).  seed=None draws a fresh seed; a seed serves ONE call."""
+    from . import SAMPLE_BELOW, SAMPLE_BITS, SAMPLE_SCALAR, EngineError, gg20, seed_words, ints_to_limbs
+    from .keygen import _buffer, _host, _upload
+    lib = eng.lib
+    if not getattr(lib, "_sample_bound", False):
+        V, S_, I_ = ctypes.c_void_p, ctypes.c_size_t, ctypes.c_int
+        lib.tecdsa_sample_batch.argtypes = [V, V, ctypes.c_uint64, ctypes.c_uint32, I_, I_, V, V, S_, I_, V, V, S_, I_]
+        lib._sample_bound = True
+    d = _descriptors(sessions, signers)
+    T, P, n = signers, keys.parties, d.shape[0]
+    E = n * T
+    N = _upload(ints_to_limbs(keys.table(0, 64), 64), mem, eng.device)         # the Paillier N of every key row
+    own = (d[:, :1] * P + d[:, 1:]).reshape(E).astype(np.uint32)
+    pos = np.arange(E) % T
+    base = np.arange(E) - pos
+    sw = seed_words(gg20.fresh_seed(seed))
+
+    def draw(out, name, kind, sub=0, rows=None, bits=0):
+        st = _buffer((E,), np.uint8, mem, eng.device)
+        ix = None if rows is None else _upload(rows, mem, eng.device)
+        eng._ck(lib.tecdsa_sample_batch(eng._ctx, _ptr(sw), sub << 32, RNDS[name], kind, bits, _ptr(N) if rows is not None else None, _ptr(ix),
+                                        0 if rows is None else N.shape[0], out.shape[-1], _ptr(out), _ptr(st), E, mem), "sample_batch")
+        bad = np.flatnonzero(_host(st))
+        if bad.size:
+            raise EngineError(f"sampling {name}: element {int(bad[0])} has status {int(_host(st)[bad[0]])}")
+
+    inp = {f: _buffer((E, w), np.uint32, mem, eng.device) for f, w in ELEMENT_FIELDS.items()}
+    inp.update({f: _buffer((T - 1, E, w), np.uint32, mem, eng.device) for f, w in PAIR_FIELDS.items()})
+    try:
+        for f in ("k", "gamma", "l", "rho", "heg_s1", "heg_s2", "dlog_nonce"):
+            draw(inp[f], f, SAMPLE_SCALAR)
+        for f in ("blind", "blind5", "blind5c"):
+            draw(inp[f], f, SAMPLE_BITS, bits=256)
+        draw(inp["r_a"], "r_a", SAMPLE_BELOW, rows=own)
+        for j in range(T - 1):
+            peer = own[base + np.where(j < pos, j, j + 1)].astype(np.uint32)
+            for f in ("beta_tag_gamma", "r_gamma", "beta_tag_w", "r_w"):
+                draw(inp[f][j], f, SAMPLE_BELOW, j, rows=peer)
+            for f in ("nonce_gamma_b", "nonce_gamma_beta", "nonce_w_b", "nonce_w_beta"):
+                draw(inp[f][j], f, SAMPLE_SCALAR, j)
+    finally:
+        sw[:] = 0
+    return inp
+
+
+def sign_device(eng: Engine, keys, signers: int, sessions, message, inp, mem: int = HOST, out=None, check: bool = True):
+    """GG18 signing (gg_2018/test.rs `sign`: phases 1-5, output_signature, verify) for every session as ONE call
+    (tecdsa_gg18_signing_batch).  sessions = [n][1 + signers]; message = [n] ints (reduced mod q) or an [n][8] limb array;
+    inp = the dict `sample_inputs` returns (or the same fields from elsewhere).  -> dict(status [E], R [E][16], r [n][8], s [n][8],
+    recid [n], complete [n]): numpy arrays for HOST, CUDA tensors for DEVICE (the caller's, when `out` holds them under the names
+    of tecdsa_gg18_signing_out; sessions and message are then CUDA tensors too).  A session that did not complete has zero R and
+    signature.  check=False returns the call's rc instead of raising."""
+    from .keygen import _buffer
+    lib = eng.lib
+    if not getattr(lib, "_gg18_signing_bound", False):
+        V = ctypes.c_void_p
+        lib.tecdsa_gg18_signing_batch.argtypes = [V, V, ctypes.c_int, ctypes.c_size_t, ctypes.c_int, V, V, ctypes.POINTER(_SigningIn),
+                                                  ctypes.POINTER(_SigningOut)]
+        lib._gg18_signing_bound = True
+    if isinstance(message, (list, tuple)):
+        message = ints_to_limbs([int(m) for m in message], 8)
+    if mem == HOST:
+        sessions = _descriptors(sessions, signers)
+        inp = {f: None if v is None else np.ascontiguousarray(v, dtype=np.uint32) for f, v in inp.items()}
+        message = np.ascontiguousarray(message, dtype=np.uint32)
+    n = sessions.shape[0]
+    E = n * signers
+    if out is None:
+        out = {"status": _buffer((E,), np.uint8, mem, eng.device), "R": _buffer((E, 16), np.uint32, mem, eng.device),
+               "sig_r": _buffer((n, 8), np.uint32, mem, eng.device), "sig_s": _buffer((n, 8), np.uint32, mem, eng.device),
+               "recid": _buffer((n,), np.uint8, mem, eng.device), "complete": _buffer((n,), np.uint8, mem, eng.device)}
+    si = _SigningIn(*[_ptr(inp[f]) for f in IN_FIELDS])
+    so = _SigningOut(*[_ptr(out[f]) for f in OUT_FIELDS])
+    rc = lib.tecdsa_gg18_signing_batch(eng._ctx, keys.handle, signers, n, mem, _ptr(sessions), _ptr(message), ctypes.byref(si), ctypes.byref(so))
+    if not check:
+        return rc
+    eng._ck(rc, "gg18_signing_batch")
+    return {"status": out["status"], "R": out["R"], "r": out["sig_r"], "s": out["sig_s"], "recid": out["recid"], "complete": out["complete"]}
