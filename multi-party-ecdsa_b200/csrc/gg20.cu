@@ -61,7 +61,7 @@ struct Builder {
 
     static void reset(ExpLaunch& l) { l.n_classes = 0; l.total_items = 0; }
     static void reset(InvLaunch& l) { l.n_classes = 0; l.total_items = 0; }
-    // Jobs modulo a square whose root the key tables hold (N^2, and the unit's own p^2 / q^2) are routed to the N-adic
+    // Jobs modulo a square whose root the key tables hold (N^2, p^2 / q^2) are routed to the N-adic
     // lists (nadic.cuh: same value, about half the MACs of the double-width Montgomery product); `l` / `gpw` then only say
     // where the class would have gone otherwise.
     void exp_class(ExpLaunch& l, int gpw, Operand mod, int nb, Operand b0, Operand e0, int el0, Operand b1, Operand e1, int el1,
@@ -101,20 +101,25 @@ struct Builder {
         ExpClass& k = l.cls[l.n_classes - 1];
         k.fb = ks->fb; k.fb_row = Operand{nullptr, rows, 0, 1, 0}; k.fb_sel[0] = 1; k.fb_sel[1] = 0;
     }
-    // own-key power base^N mod N^2 (the unit knows its own p, q), slot s, in three stages (declared shortcut: identical
-    // value): b^(pq) mod p^2 == ((b mod p)^(q mod (p-1)) mod p)^p mod p^2 because x^p mod p^2 depends only on x mod p.
-    //   1. 1024-bit job list:  TP[s] = (b mod p)^(q mod (p-1)) mod p,   TQ[s] likewise          (crt_stage1)
-    //   2. 2048-bit job list:  YP[s] = TP[s]^p mod p^2,  YQ[s] = TQ[s]^q mod q^2                (crt_stage2)
-    //   3. gg20_crt recombines YP, YQ into XC[s] in [0, N^2)
+    // power base^N mod N^2 under key row rows[u] (the unit's own, or its peer's: the fused call holds the factors of both),
+    // slot s, in three stages (declared shortcuts 5 and 12: identical value for every b): b^(pq) mod p^2 ==
+    // ((b mod p)^(q mod (p-1)) mod p)^p mod p^2 because x^p mod p^2 depends only on x mod p, and q mod (p-1) != 0.
+    //   1. 1024-bit job list:  TP[s] = (b mod p)^(q mod (p-1)) mod p,   TQ[s] likewise                     (crt_stage1)
+    //   2. p-adic job list:    YP[s] = TP[s]^p [* b1^e1 * m0] mod p^2,  YQ[s] = TQ[s]^q [* b1^e1 * m0] mod q^2  (crt_stage2)
+    //   3. gg20_crt recombines YP, YQ into a field in [0, N^2)
+    // The optional second base b1 and multiplier m0 (plain operands up to 4K limbs, reduced by the p-adic lift) make stage 2
+    // one Straus job for a product of the N-th power with further factors mod N^2.
     void crt_stage1(ExpLaunch& l32, int gpw32, const uint32_t* rows, int slot, Operand base64) {
         const Operand none = {nullptr, nullptr, 0, 0, 0};
         exp_class(l32, gpw32, key(KT_P, rows), 1, base64, key(KT_QMODPM1, rows), 32, none, none, 0, 0, none, none, F_TP0 + slot, 1);
         exp_class(l32, gpw32, key(KT_Q, rows), 1, base64, key(KT_PMODQM1, rows), 32, none, none, 0, 0, none, none, F_TQ0 + slot, 1);
     }
-    void crt_stage2(ExpLaunch& l64, int gpw64, const uint32_t* rows, int slot) {
+    void crt_stage2(ExpLaunch& l64, int gpw64, const uint32_t* rows, int slot, Operand b1 = Operand{nullptr, nullptr, 0, 0, 0},
+                    Operand e1 = Operand{nullptr, nullptr, 0, 0, 0}, int el1 = 0, Operand m0 = Operand{nullptr, nullptr, 0, 0, 0}) {
         const Operand none = {nullptr, nullptr, 0, 0, 0};
-        exp_class(l64, gpw64, key(KT_PP, rows), 1, fld(F_TP0 + slot, 32), key(KT_P, rows), 32, none, none, 0, 0, none, none, F_YP0 + slot);
-        exp_class(l64, gpw64, key(KT_QQ, rows), 1, fld(F_TQ0 + slot, 32), key(KT_Q, rows), 32, none, none, 0, 0, none, none, F_YQ0 + slot);
+        const int nb = b1.ptr ? 2 : 1, nm = m0.ptr ? 1 : 0;
+        exp_class(l64, gpw64, key(KT_PP, rows), nb, fld(F_TP0 + slot, 32), key(KT_P, rows), 32, b1, e1, el1, nm, m0, none, F_YP0 + slot);
+        exp_class(l64, gpw64, key(KT_QQ, rows), nb, fld(F_TQ0 + slot, 32), key(KT_Q, rows), 32, b1, e1, el1, nm, m0, none, F_YQ0 + slot);
     }
     void inv_class(InvLaunch& l, int gpw, Operand mod, Operand in, int out_field, int flag_byte) {
         InvLaunch* dst = &l;
@@ -147,9 +152,9 @@ template <typename Kern> int glue_named(tecdsa_ctx* c, Kern kern, const char* na
     return e == cudaSuccess ? 0 : tecdsa_fail(TECDSA_E_CUDA, "glue launch", e);
 }
 
-int glue_crt(tecdsa_ctx* c, const Arena& A, int first, int count) {
+int glue_crt(tecdsa_ctx* c, const Arena& A, const uint32_t* rows, int first, int count, int dst) {
     c->prof_begin("gg20_crt");
-    gg20_crt<<<(A.U + 63) / 64, 64, 0, c->stream>>>(A, first, count);
+    gg20_crt<<<(A.U + 63) / 64, 64, 0, c->stream>>>(A, rows, first, count, dst);
     c->prof_end();
     c->count_launch();
     cudaError_t e = cudaGetLastError();
@@ -389,7 +394,7 @@ static int offline_impl(tecdsa_ctx* c, const tecdsa_keyset* ks, const uint32_t* 
         B.fb_class(L64, GPW64, st_rows(x), B.rnd(al + RND_AL_RHO, 72), 72, B.rnd(RND_K, 8), 8, 0, NONE, F_Z0 + x);
     }
     RUN(run_exp(c, B.LPQ, -32)); RUN(run_exp(c, L64, 64));
-    RUN(glue_crt(c, A, 0, 4));
+    RUN(glue_crt(c, A, ro, 0, 4, F_XC0));
     B.exp_class(L128, GPW128, B.key(KT_NN, ro), 0, NONE, NONE, 0, NONE, NONE, 0, 2, B.fld(F_MK), B.fld(F_XC0), F_CK);
     for (int x = 0; x < 3; x++)
         B.exp_class(L128, GPW128, B.key(KT_NN, ro), 0, NONE, NONE, 0, NONE, NONE, 0, 2, B.fld(F_ALIN0 + x), B.fld(F_XC1 + x), F_U0 + x);
@@ -410,21 +415,24 @@ static int offline_impl(tecdsa_ctx* c, const tecdsa_keyset* ks, const uint32_t* 
     RUN(run_inv(c, I128, 128)); RUN(run_inv(c, B.I128H, -128));
     for (int x = 0; x < 3; x++)
         B.exp_class(L64, GPW64, B.key(KT_NT, st_rows(x)), 1, B.peer(F_Z0 + x), B.peer(F_E0 + x), 8, NONE, NONE, 0, 0, NONE, NONE, F_ZE0 + x);   // z^e (:122)
-    RUN(run_exp(c, L64, 64));
+    // s^N of u' (below) under the PEER's key through CRT halves: the fused call holds the factors of every key row (declared
+    // shortcut 12), slots 6..8, first stage
+    for (int x = 0; x < 3; x++) B.crt_stage1(L32, GPW32, rp, 6 + x, B.peer(F_S0 + x, 64));
+    RUN(run_exp(c, L32, 32)); RUN(run_exp(c, L64, 64));
     for (int x = 0; x < 3; x++) B.inv_class(I64, GPW64, B.key(KT_NT, st_rows(x)), B.fld(F_ZE0 + x), F_ZEI0 + x, x);
     RUN(run_inv(c, I64, 64));
     for (int x = 0; x < 3; x++) {
         // w' = h1^s1 * h2^s2 * (z^e)^-1 mod N_tilde                     (range_proofs.rs:129-132)
         B.fb_class(L64, GPW64, st_rows(x), B.peer(F_S20 + x), 92, B.peer(F_S10 + x), 28, 1, B.fld(F_ZEI0 + x), F_WV0 + x);
-        // u' = (s1 N + 1) * s^N * (c^e)^-1 mod N^2                      (range_proofs.rs:134-141); (c^-1)^e (:135) is the second
-        // base of the same job and shares its squarings
-        B.exp_class(L128, GPW128, B.key(KT_NN, rp), 2, B.peer(F_S0 + x, 64), B.key(KT_N, rp), 64, B.fld(F_CINVP), B.peer(F_E0 + x), 8, 1,
-                    B.fld(F_GS10 + x), NONE, F_UV0 + x);
+        // u' = (s1 N + 1) * s^N * (c^e)^-1 mod N^2                      (range_proofs.rs:134-141) as its halves mod p^2, q^2 of the
+        // peer's key: TP^p * (c^-1)^e * (s1 N + 1); (c^-1)^e (:135) is the second base of the same job and shares its squarings
+        B.crt_stage2(L64, GPW64, rp, 6 + x, B.fld(F_CINVP), B.peer(F_E0 + x), 8, B.fld(F_GS10 + x));
     }
     // c_b = c_a^b * Enc(beta'; r') mod N^2 for b = gamma_i and b = w_i  (mta/mod.rs:133-145)
     B.exp_class(L128, GPW128, B.key(KT_NN, rp), 2, B.rnd(RND_R_G, 64), B.key(KT_N, rp), 64, B.peer(F_CK), B.rnd(RND_GAMMA, 8), 8, 1, B.fld(F_LBG), NONE, F_CBG);
     B.exp_class(L128, GPW128, B.key(KT_NN, rp), 2, B.rnd(RND_R_W, 64), B.key(KT_N, rp), 64, B.peer(F_CK), B.fld(F_W), 8, 1, B.fld(F_LBW), NONE, F_CBW);
     RUN(run_exp(c, L128, 128)); RUN(run_exp(c, B.LPQ, -32)); RUN(run_exp(c, L64, 64));
+    RUN(glue_crt(c, A, rp, 6, 3, F_UV0));
     RUN(glue(c, gg20_r1_post_hash, A, 3));
     RUN(glue(c, gg20_r1_post_dlog, A, 4));
 
@@ -449,7 +457,7 @@ static int offline_impl(tecdsa_ctx* c, const tecdsa_keyset* ks, const uint32_t* 
     RUN(run_exp(c, L32, 32));
     B.crt_stage2(L64, GPW64, ro, 4);
     RUN(run_exp(c, B.LPQ, -32)); RUN(run_exp(c, L64, 64));
-    RUN(glue_crt(c, A, 4, 1));
+    RUN(glue_crt(c, A, ro, 4, 1, F_XC4));
     B.exp_class(L128, GPW128, B.key(KT_NN, ro), 0, NONE, NONE, 0, NONE, NONE, 0, 2, B.fld(F_PLIN), B.fld(F_XC4), F_PU2);
     RUN(run_exp(c, L128, 128));
     RUN(glue(c, gg20_r4_mid, A));
@@ -469,7 +477,7 @@ static int offline_impl(tecdsa_ctx* c, const tecdsa_keyset* ks, const uint32_t* 
     RUN(run_exp(c, L32, 32));
     B.crt_stage2(L64, GPW64, ro, 5);
     RUN(run_exp(c, L128, 128)); RUN(run_exp(c, B.LPQ, -32)); RUN(run_exp(c, L64, 64));
-    RUN(glue_crt(c, A, 5, 1));
+    RUN(glue_crt(c, A, ro, 5, 1, F_XC5));
     B.inv_class(I64, GPW64, B.key(KT_NT, rp), B.fld(F_VZE0), F_VZEI0, 6);
     RUN(run_inv(c, I64, 64));
     // u3' = h1^s1 * h2^s3 * z^-e mod N_tilde                             (:158-172)

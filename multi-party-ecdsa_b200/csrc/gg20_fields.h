@@ -52,13 +52,14 @@ enum : int {
     X(DIGEST, 8)                                                                                  \
     X(FLAGS, 8)                                     /* one ok byte per check, see gg20_glue.cuh */          \
     X(DBG, 256)                                     /* scratch for tools/debug_gg20.py */            \
-    /* own-key powers b^N mod N^2 through CRT: halves mod p^2 / q^2 and the recombined value */      \
-    X(YP0, 64) X(YP1, 64) X(YP2, 64) X(YP3, 64) X(YP4, 64) X(YP5, 64)                              \
-    X(YQ0, 64) X(YQ1, 64) X(YQ2, 64) X(YQ3, 64) X(YQ4, 64) X(YQ5, 64)                              \
+    /* powers b^N mod N^2 through CRT: halves mod p^2 / q^2 and, for the own-key slots 0..5, the     \
+       recombined value; slots 6..8 are the peer-key u' of round 1, recombined straight into UV0..2 */ \
+    X(YP0, 64) X(YP1, 64) X(YP2, 64) X(YP3, 64) X(YP4, 64) X(YP5, 64) X(YP6, 64) X(YP7, 64) X(YP8, 64) \
+    X(YQ0, 64) X(YQ1, 64) X(YQ2, 64) X(YQ3, 64) X(YQ4, 64) X(YQ5, 64) X(YQ6, 64) X(YQ7, 64) X(YQ8, 64) \
     X(XC0, 128) X(XC1, 128) X(XC2, 128) X(XC3, 128) X(XC4, 128) X(XC5, 128)                          \
     /* 1024-bit stage: (b mod p)^(q mod (p-1)) mod p and the q-side twin */                          \
-    X(TP0, 32) X(TP1, 32) X(TP2, 32) X(TP3, 32) X(TP4, 32) X(TP5, 32)                              \
-    X(TQ0, 32) X(TQ1, 32) X(TQ2, 32) X(TQ3, 32) X(TQ4, 32) X(TQ5, 32)
+    X(TP0, 32) X(TP1, 32) X(TP2, 32) X(TP3, 32) X(TP4, 32) X(TP5, 32) X(TP6, 32) X(TP7, 32) X(TP8, 32) \
+    X(TQ0, 32) X(TQ1, 32) X(TQ2, 32) X(TQ3, 32) X(TQ4, 32) X(TQ5, 32) X(TQ6, 32) X(TQ7, 32) X(TQ8, 32)
 
 enum Field : int {
 #define X(name, size) F_##name,
@@ -90,8 +91,8 @@ enum KeyTable : int {
     KT_PINV2, KT_QINV2,  // 32   p^-1, q^-1 mod 2^1024 (exact division in the L-function)
     KT_HPR, KT_HQR,  // 32   hp*R mod p, hq*R mod q  (R = 2^1024; hp = L_p((1-N) mod p^2)^-1 mod p)
     KT_PINVQR,       // 32   (p^-1 mod q) * R mod q
-    KT_PPINVQQR,     // 64   ((p^2)^-1 mod q^2) * 2^2048 mod q^2  (CRT recombination of own-key N^2 powers)
-    KT_QMODPM1, KT_PMODQM1,   // 32   q mod (p-1), p mod (q-1): exponents of the 1024-bit stage of an own-key N-th power
+    KT_PPINVQQR,     // 64   ((p^2)^-1 mod q^2) * 2^2048 mod q^2  (CRT recombination of N^2 powers)
+    KT_QMODPM1, KT_PMODQM1,   // 32   q mod (p-1), p mod (q-1): exponents of the 1024-bit stage of an N-th power
     KT_XI,           // 8    x_i
     KT_PK,           // 16   X_i affine
     KT_COUNT

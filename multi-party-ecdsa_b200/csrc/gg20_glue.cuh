@@ -217,14 +217,16 @@ __device__ __forceinline__ void put_padded(Sha256& h, const uint32_t* limbs, int
 }
 
 
-// CRT recombination of an own-key power: x = yp + p^2 * ((yq - yp) * (p^2)^-1 mod q^2)  in [0, N^2)
+// CRT recombination of a power under key row `row` (the unit's own or its peer's): x = yp + p^2 * ((yq - yp) * (p^2)^-1 mod q^2)
+// in [0, N^2)
 static __device__ __noinline__ void crt_combine(uint32_t* x128, const Arena& A, uint32_t row, const uint32_t* yp, const uint32_t* yq) {
     const uint32_t *pp = A.k(KT_PP, row), *qq = A.k(KT_QQ, row);
     uint32_t d[65], ypr[65], qx[65], big[129];
     for (int i = 0; i < 64; i++) { d[i] = yq[i]; ypr[i] = yp[i]; qx[i] = qq[i]; }
     d[64] = 0; ypr[64] = 0; qx[64] = 0;
     st::sub(d, d, ypr, 65);
-    // p < 4q for every accepted key (see decrypt_finish), so yq - yp > -p^2 > -16 q^2: at most 16 additions
+    // p < 4q for every accepted key row, the peer's included (see decrypt_finish), so yq - yp > -p^2 > -16 q^2: at most 16
+    // additions
     for (int it = 0; it < 16 && (d[64] >> 31); it++) st::add(d, d, qx, 65);
     uint32_t t[64];
     st::mont_mul(t, d, A.k(KT_PPINVQQR, row), qq, st::neg_inv32_st(qq[0]), 64, big);

@@ -405,12 +405,13 @@ static __global__ void gg20_key_setup(uint32_t* const* tables, int rows) {
     }
 }
 
-// recombine `count` (1..4) consecutive (YP, YQ) field pairs starting at slot `first` into XC
-static __global__ void gg20_crt(Arena A, int first, int count) {
+// recombine `count` (1..4) consecutive (YP, YQ) field pairs starting at slot `first` under the key row rows[u] (the unit's own
+// or its peer's) into the consecutive fields starting at `dst`
+static __global__ void gg20_crt(Arena A, const uint32_t* rows, int first, int count, int dst) {
     int u = blockIdx.x * blockDim.x + threadIdx.x;
     if (u >= A.U) return;
-    const uint32_t row = A.row_own[u];
-    for (int s = first; s < first + count; s++) crt_combine(A.p(F_XC0 + s, u), A, row, A.p(F_YP0 + s, u), A.p(F_YQ0 + s, u));
+    const uint32_t row = rows[u];
+    for (int s = 0; s < count; s++) crt_combine(A.p(dst + s, u), A, row, A.p(F_YP0 + first + s, u), A.p(F_YQ0 + first + s, u));
 }
 
 }  // namespace tecdsa
